@@ -39,12 +39,8 @@ SIGNATURES = {
     'di_lcab_window_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_lcab_window_pre_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p],
     'di_lcab_window_tc_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p],
-    'di_lcab_window_tc_set_sm_limit': [_i],
-    'di_lcab_window_tc_set_debug': [_i],
-    'di_lcab_window_tc_debug_read': [ctypes.POINTER(ctypes.c_longlong)],
     'di_lcab_proj_f32': [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p],
     'di_lcab_forward_f32': [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p],
-    'di_lcab_proj_set_sm_limit': [_i],
     'di_set_window_ffma': [_i],
     'di_locatt_cc2k_f32': [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_locatt_ck2c_ori_f32': [_p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
@@ -126,7 +122,7 @@ def lib():
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(
                 f'{LIB_PATH} not found: build it with `python -m deepinteraction_b200.build` '
-                '(nvcc, sm_100a).  There is no CPU/PyTorch fallback for the MMRI/MMPI kernels.')
+                '(nvcc, sm_90a).  There is no CPU/PyTorch fallback for the MMRI/MMPI kernels.')
         L = ctypes.CDLL(LIB_PATH)
         L.di_last_error.restype = ctypes.c_char_p
         L.di_last_error.argtypes = []

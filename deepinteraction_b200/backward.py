@@ -9,7 +9,7 @@ form the forward kernels use): d/d target map, d/d source map, d/d folded weight
 The gradient of a folded weight maps to the convolution weight by the BN scale (dW_conv = dW_folded * gamma / sqrt(var +
 eps)), and d beta = d bias_folded.  Train-mode BatchNorm (batch statistics with their own gradient) and dropout are not
 covered.  The intermediates are recomputed in fp32 (q1, k1, q, k, v and the [P, 81] attention weights), the window
-products run in the unfused kernels of csrc/lcab_bwd.cu, dense products on the tcgen05 / FFMA GEMMs.
+products run in the unfused kernels of csrc/lcab_bwd.cu, dense products on the wgmma / FFMA GEMMs.
 """
 import torch
 

@@ -1,8 +1,8 @@
-"""Build libdi_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Build libdi_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a (H100).
 
     python -m deepinteraction_b200.build [--force]
 
-The library is compiled for sm_100a ONLY (-gencode arch=compute_100a,code=sm_100a): there is no
+The library is compiled for sm_90a ONLY (-gencode arch=compute_90a,code=sm_90a): there is no
 other backend and no CPU fallback.  nvcc cross-compiles without a GPU.
 """
 import glob
@@ -13,7 +13,7 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libdi_b200.so')
-NVCC_FLAGS = ['-gencode', 'arch=compute_100a,code=sm_100a', '-O3', '-lineinfo', '-std=c++17',
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-O3', '-lineinfo', '-std=c++17',
               '-Xcompiler', '-fPIC', '--expt-relaxed-constexpr']
 
 

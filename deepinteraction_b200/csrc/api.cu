@@ -17,7 +17,7 @@ const char* di_last_error(void) { return g_err; }
 
 int di_version(void) { return 100; }
 
-// Compute capability the library was built for (major*10+minor); the kernels use sm_100a only.
-int di_built_arch(void) { return 100; }
+// Compute capability the library was built for (major*10+minor); the kernels use sm_90a only.
+int di_built_arch(void) { return 90; }
 
 }  // extern "C"

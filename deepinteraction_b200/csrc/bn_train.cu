@@ -7,7 +7,7 @@
 
 namespace {
 
-constexpr int BN_BLOCKS = 592;   // 4 x 148 row blocks
+constexpr int BN_BLOCKS = 528;   // 4 x 132 row blocks (H100 SXM)
 
 __device__ __forceinline__ float4 ld4(const float* p) { return __ldg(reinterpret_cast<const float4*>(p)); }
 inline int bn_blocks(long long M) { return (int)(M < BN_BLOCKS ? M : BN_BLOCKS); }

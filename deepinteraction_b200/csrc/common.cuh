@@ -1,4 +1,4 @@
-// Shared helpers for the sm_100a kernels of libdi_b200.
+// Shared helpers for the sm_90a kernels of libdi_b200.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

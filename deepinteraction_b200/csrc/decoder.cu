@@ -497,8 +497,8 @@ rows_finish_c128_kernel(const float* __restrict__ x, int ldx, const float* __res
 
 
 // ------------------------------------------------------------------------------------------------
-// Query-row MLP: the decoder runs dozens of dense layers on B*P = 200..600 query rows.  On the tcgen05 path each is a
-// 20 us launch dominated by start-up (TMEM allocation, tensor maps, barrier set-up); here one CTA takes 4 rows through
+// Query-row MLP: the decoder runs dozens of dense layers on B*P = 200..600 query rows.  On the tensor-core GEMM each is a
+// launch dominated by start-up (tensor maps, barrier set-up); here one CTA takes 4 rows through
 // up to TWO chained dense layers, a residual, a LayerNorm and an activation without leaving shared memory:
 //     H = act1([X0 | X1] W1^T + b1)            Y = H W2^T + b2   (or Y = H)
 //     Y = act_out(LN(Y + res))                 rows with zero_if_neg[m] < 0 are written as 0
@@ -513,8 +513,7 @@ constexpr int MLP_CHUNK = 8192; // floats per stage (32 KB): KC = 8192 / N conse
 
 // Weight streaming: the [K, N] transposed weights are contiguous, so KC rows are one 32 KB block; every thread copies
 // 16-byte pieces of it with cp.async into a 5-stage ring (128 KB in flight per CTA; layer 2's first chunks are under way
-// while layer 1 still computes).  Measured alternatives: dependent batches of __ldg (K / 16 round trips per layer:
-// 25-45 us per launch) and one cp.async.bulk per chunk (the copy engine delivered ~32 GB/s per SM).
+// while layer 1 still computes), instead of dependent batches of __ldg (K / 16 round trips per layer).
 __device__ __forceinline__ void mlp_copy_chunk(float* dst, const float* src, int floats, int tid) {
   const uint32_t d = tc::smem_u32(dst);
   for (int i = tid * 4; i < floats; i += MLP_NT * 4)
@@ -944,7 +943,7 @@ dynconv_kernel(const float* __restrict__ roi, const float* __restrict__ params, 
   const int qn = blockIdx.x, t = threadIdx.x;
   // the query's two 128 x 128 parameter matrices (128 KB, written by the generator GEMM just before) are pulled into
   // shared memory with cp.async while the RoI tile loads: reading them with dependent __ldg batches inside the product
-  // loop left the kernel latency-bound (57 us for 26 MB)
+  // loop leaves the kernel latency-bound
   float* PS = dyn_smem + 2 * DR * DC;                    // [2][DC][DC]
   {
     const float* psrc = params + (size_t)qn * 2 * DC * DC;

@@ -1,5 +1,5 @@
-// Blackwell tensor-core path of the dense layers: C[M,N] = act(A[M,K] * W[N,K]^T + bias (+res)), fp32 in/out,
-// computed as an error-compensated SPLIT product on tcgen05 (UMMA) with the accumulator in tensor memory:
+// Hopper tensor-core path of the dense layers: C[M,N] = act(A[M,K] * W[N,K]^T + bias (+res)), fp32 in/out,
+// computed as an error-compensated SPLIT product on warpgroup MMA (wgmma) with fp32 accumulators in registers:
 //
 //     A = A_hi + A_lo,  W = W_hi + W_lo,    A*W ~= A_hi*W_hi + A_lo*W_hi + A_hi*W_lo
 //
@@ -10,71 +10,28 @@
 // models/necks/deepinteraction_encoder.py:26-32) and the 3x3 convs as implicit GEMM over pixel-major (NHWC) maps
 // (models/necks/deepinteraction_encoder.py:47-62, models/dense_heads/deepinteraction_decoder.py:83-101).
 //
-// Persistent CTAs (one per SM) take 128 x 128 output tiles from a global atomic counter; 320 threads,
-// warp-specialised, all hand-offs through mbarriers:
-//   warp 0      TMA producer: tile ids (atomics, published through a shared-memory queue, L2 prefetch of the next
-//               tiles' A rows) and, per K chunk, box loads of fp32 A (2-D [rows,K] map, or a 4-D NHWC map whose
-//               8x16-pixel box shifted by the filter tap gives the zero padding for free) and of W_hi / W_lo into a
-//               ring of 128B-swizzled K-major tiles (cp.async.bulk.tensor + mbarrier tx-count).  For K <= 128 the
-//               weight slice is loaded once and stays resident.
-//   warps 2-5   splitter: landed A chunk -> registers -> hi / lo -> tcgen05.st into TENSOR MEMORY (A never goes
-//               back to shared memory)
-//   warp 1      MMA issuer (elect.sync): per chunk 4 k-steps x 3 products of tcgen05.mma (M=128, N=128), A operand
-//               from TMEM, W from shared memory; one tcgen05.commit per chunk releases the A buffer and the stage
-//   warps 6-9   epilogue: tcgen05.ld (two 32-column loads in flight) -> bias / residual / activation -> 128B-
-//               swizzled staging buffer -> cp.async.bulk.tensor store; overlaps the next tile's main loop through
-//               a double-buffered accumulator
-//   TMEM columns: [0,128) acc0 | [128,256) acc1 | [256 + 64 b, +64) A buffer b (hi 32 | lo 32)
+// Persistent CTAs (at most one per SM) walk the 128 x 128 output tiles with a static stride; 384 threads in three
+// warpgroups, all hand-offs through mbarriers:
+//   warpgroup 0   TMA producer (one thread): per K chunk, box loads of fp32 A (2-D [rows,K] map, or a 4-D NHWC map
+//                 whose 8x16-pixel box shifted by the filter tap gives the zero padding for free) and of W_hi / W_lo
+//                 into a ring of 128B-swizzled K-major tiles (cp.async.bulk.tensor + mbarrier tx-count); L2 prefetch of
+//                 the next tile's A rows.  For K <= 128 the weight slice is loaded once and stays resident.
+//   warpgroups 1-2  consumers, 64 output rows each: landed A chunk -> registers (the wgmma A fragment, read through
+//                 the swizzle) -> hi / lo split in registers -> wgmma with W_hi / W_lo straight from shared memory;
+//                 then the epilogue from the accumulator registers: bias / residual / activation -> global stores.
 #include "tc_common.cuh"
-#include <mutex>
-#include <vector>
-
-// ------------------------------------------------------------------------------------------------
-// Dynamic tile-scheduler state of the persistent tensor-core kernels (this file and lcab_tc.cu): every launch gets
-// a 16-int slot (tile counters + a done counter); the last CTA of a launch zeroes its slot again.  Slots come from a
-// ring that belongs to the (device, stream) pair of the launch: launches of one stream are serialised, so a slot can
-// only ever be shared by launches that cannot overlap -- also under graph replay, where the slot address is baked
-// into the captured launch and the graph is replayed on the stream it was captured on (graph.GraphCache keys on the
-// stream).  Launches of different streams (frames in flight, pipeline.FramePipeline) never share a slot.
-// ------------------------------------------------------------------------------------------------
-namespace tc {
-constexpr int SCHED_RINGS = 64, SCHED_RING_SLOTS = 64;
-__device__ int g_sched_pool[SCHED_RINGS * SCHED_RING_SLOTS * 16];
-struct Ring { int dev; cudaStream_t stream; unsigned seq; };
-static std::mutex g_sched_mu;
-static std::vector<Ring> g_rings;
-static int* g_pool_ptr[64] = {nullptr};
-
-int* sched_slot(cudaStream_t stream) {
-  int dev = 0;
-  cudaGetDevice(&dev);
-  if (dev < 0 || dev >= 64) return nullptr;
-  std::lock_guard<std::mutex> lock(g_sched_mu);
-  if (!g_pool_ptr[dev] && cudaGetSymbolAddress(reinterpret_cast<void**>(&g_pool_ptr[dev]), g_sched_pool) != cudaSuccess)
-    return nullptr;
-  size_t r = 0;
-  for (; r < g_rings.size(); ++r)
-    if (g_rings[r].dev == dev && g_rings[r].stream == stream) break;
-  if (r == g_rings.size()) g_rings.push_back(Ring{dev, stream, 0u});
-  // more than SCHED_RINGS (device, stream) pairs: rings are reused modulo SCHED_RINGS (documented limit)
-  const size_t ring = r % SCHED_RINGS;
-  const unsigned slot = g_rings[r].seq++ % SCHED_RING_SLOTS;
-  return g_pool_ptr[dev] + (ring * SCHED_RING_SLOTS + slot) * 16;
-}
-}  // namespace tc
 
 namespace {
 
 constexpr int TM = 128, TN = 128, TK = 32;          // tile; TK fp32 = 128 bytes = one swizzle row
-constexpr int A_BYTES = TM * TK * 4;                // 16 KB
-constexpr int NTHREADS = 320;
-constexpr int EP_BYTES = 4 /*warps*/ * 2 /*buffers*/ * 32 * 128;   // epilogue staging: 32 rows x 128 B per buffer
+constexpr int A_BYTES = TM * TK * 4;                // 16 KB: one 128-row x 128-byte operand box
+constexpr int NTHREADS = 384;
+constexpr int RING_BYTES = 192 * 1024;
+constexpr int BAR_BYTES = 256;
+constexpr int V3_SMEM_BYTES = RING_BYTES + 1024 /*alignment*/ + BAR_BYTES;
+static_assert(V3_SMEM_BYTES <= 232448, "gemm_tc exceeds the 227 KB shared-memory limit");
 
 using namespace tc;
-
-// kind::tf32, fp32 accumulate, A and B K-major, M = 128, N = 128
-constexpr uint32_t IDESC = (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-
 
 // optional pipeline trace (CTA 0 only): clock64 stamps per role and chunk, read back with di_tc_debug_read
 constexpr int DBG_SLOTS = 8, DBG_N = 512;
@@ -84,24 +41,10 @@ __device__ long long g_dbg[DBG_SLOTS * DBG_N];
     if (p.dbg && blockIdx.x == 0 && (i) < DBG_N) g_dbg[(slot) * DBG_N + (i)] = clock64(); \
   } while (0)
 
-// Activation over a register tile with ONE warp-uniform branch.  (Calling di_act per element made ptxas
-// if-convert the GELU polynomial: every element paid ~60 predicated-off instructions, 3000 cycles per 32-column
-// epilogue step -- found with the clock64 trace.)
-__device__ __forceinline__ void act_tile(float (&v)[32], int act) {
-  if (act == DI_ACT_RELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = fmaxf(v[j], 0.f);
-  } else if (act == DI_ACT_GELU) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) v[j] = 0.5f * v[j] * (1.f + erff(v[j] * 0.70710678118654752440f));
-  }
-}
-
-
 struct TcParams {
   int M, N;                 // logical output size (rows, columns)
   int nsrc;                 // linear: number of A sources (1..3)
-  int k0, k1, k2;           // linear: K_s / 32 per source; conv: k0 = Cin / 32.  (Scalars, not an array: a dynamically
+  int k0, k1, k2;           // linear: K_s / KE per source; conv: k0 = Cin / KE.  (Scalars, not an array: a dynamically
                             // indexed kernel parameter makes ptxas copy the whole struct to LOCAL memory.)
   int conv;                 // 1: 3x3 conv over an NHWC map (A map is 4-D)
   int H, W, tiles_x, tiles_y;  // conv geometry: tile = 8 rows x 16 cols of pixels
@@ -112,136 +55,67 @@ struct TcParams {
   const float* res;
   int ldres, res_mod, act;
   int dbg;
-  int* sched;               // v3: 16 ints of the dynamic tile scheduler (column-group counters [0..13], done [15])
   int split_col0, split_kind;  // output columns >= split_col0 are emitted as bf16 (hi, mid) words (0 = off), see below
   int a_nchw;               // conv: the input map is NCHW (kernel variant ANCHW)
 };
 __host__ __device__ __forceinline__ int tc_kch(const TcParams& p, int s) { return s == 0 ? p.k0 : (s == 1 ? p.k1 : p.k2); }
 
-// ------------------------------------------------------------------------------------------------
-// v3: A operand through TENSOR MEMORY.  Shared-memory bandwidth is the limiter of the 3xTF32 scheme (every
-// k-step re-reads A_hi twice, A_lo once and W_hi twice, W_lo once from shared memory, on top of the TMA writes,
-// the splitter's round trip and the epilogue staging -- measured 896 KB of smem traffic per 128x128x128 tile).
-// Here the splitter reads the landed A chunk once, and writes A_hi / A_lo with tcgen05.st into TMEM; the MMA
-// takes A from TMEM ([a_tmem]) and only W from shared memory.  That removes the A_hi/A_lo write-back (128 KB
-// per tile) and the A operand reads (192 KB per tile), and frees room for a 4th pipeline stage.
-//   TMEM columns: [0,128) acc0 | [128,256) acc1 | [256 + 64 b, +64) A buffer b = 0..3 (hi 32 | lo 32)
-// ------------------------------------------------------------------------------------------------
-//
 // Two operand precisions share this kernel (template flag BF):
-//   BF = false  "3xTF32": x = hi + lo with hi = tf32(x); products A_lo W_hi + A_hi W_lo + A_hi W_hi on kind::tf32
-//               (K = 8 per instruction), 32 k-values per pipeline chunk.  Error ~2^-21 per product.
+//   BF = false  "3xTF32" (the PRECISE mode): x = hi + lo with hi = tf32(x); products A_hi W_hi into the main
+//               accumulator, A_lo W_hi + A_hi W_lo into a second one that is added in the epilogue (the tensor core
+//               truncates at every accumulate, so the main product's error grows with the number of instructions that
+//               hit its accumulator); wgmma k8, 32 k-values per pipeline chunk.  Error ~2^-21 per product.
 //   BF = true   "bf16 split": x = hi + mid with hi = bf16(x), mid = bf16(x - hi) (16 mantissa bits kept);
-//               products A_mid W_hi + A_hi W_mid + A_hi W_hi on kind::f16 (K = 16 per instruction), 64 k-values
-//               per chunk.  Error ~3 * 2^-18 per product (1e-5), far inside the 1e-3 budget of the path, for HALF
-//               the tensor-pipe time, half the tensor-memory writes and half the weight bytes per k.
-// Chunk geometry is chosen so that both variants use the same operand tiles: a weight chunk is 128 rows x 128 B
-// (32 tf32 or 64 bf16), an A chunk occupies 32 + 32 TMEM columns, and one chunk is 4 MMA k-steps of 32 bytes.
-constexpr int V3_TQ = 8;                             // depth of the in-CTA tile-id queue
-constexpr int V3_BAR_BYTES = 512;
-constexpr int V3_SMEM_BYTES = 192 * 1024 + EP_BYTES + 1024 + V3_BAR_BYTES + 512 /*bias*/ + 64 /*tile queue*/;
-static_assert(V3_SMEM_BYTES <= 232448, "v3 exceeds the 227 KB shared-memory limit");
-// kind::f16, bf16 x bf16 -> fp32, A and B K-major, M = 128, N = 128
-constexpr uint32_t IDESC_BF16 = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(TN >> 3) << 17) | ((uint32_t)(TM >> 4) << 24);
-
-
-// Pre-split outputs for the window-attention kernel (lcab.cu), same 4 bytes per value, same position of each
-// 32-channel block: the consumer then needs no conversion pass.  hi = bf16(x), mid = bf16(x - hi), packed bf16x2
-// with the lower channel in the low half.
-//   kind 1 (Q, K): channel pair (2j, 2j+1) -> words 2j = hi pair, 2j+1 = mid pair          (one LDS.64 per fragment)
-//   kind 2 (V):    channel group of 8      -> words 8g..8g+3 = hi pairs, 8g+4..8g+7 = mid pairs  (16-byte rows for
-//                                             ldmatrix.trans: the k index of P V is the key, not the channel)
-//   kind 3 (planar, tcgen05 window kernel): group of 128 channels -> 64 hi words | 64 mid words (finish_pair_planar)
-__device__ __forceinline__ void split_block(float (&v)[32], int kind) {
-  if (kind == 1) {
-#pragma unroll
-    for (int j = 0; j < 16; ++j) {
-      const uint32_t h = pack_bf16x2(v[2 * j], v[2 * j + 1]);
-      const uint32_t m = pack_bf16x2(v[2 * j] - __uint_as_float(h << 16), v[2 * j + 1] - __uint_as_float(h & 0xFFFF0000u));
-      v[2 * j] = __uint_as_float(h);
-      v[2 * j + 1] = __uint_as_float(m);
-    }
-  } else {
-#pragma unroll
-    for (int g = 0; g < 4; ++g) {
-      uint32_t h[4], m[4];
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        const float a = v[8 * g + 2 * q], b = v[8 * g + 2 * q + 1];
-        h[q] = pack_bf16x2(a, b);
-        m[q] = pack_bf16x2(a - __uint_as_float(h[q] << 16), b - __uint_as_float(h[q] & 0xFFFF0000u));
-      }
-#pragma unroll
-      for (int q = 0; q < 4; ++q) {
-        v[8 * g + q] = __uint_as_float(h[q]);
-        v[8 * g + 4 + q] = __uint_as_float(m[q]);
-      }
-    }
-  }
-}
-
-// WRES: the whole [128, K<=128] weight slice (hi + lo, <= 128 KB) of this CTA's column tile stays resident in
-// shared memory; only A streams.  The SM<->L2 port (~28 B/clk/SM, shared by loads and stores) is what bounds the
-// K=128 layers: per 128x128 tile it moves 64 KB (A) + 64 KB (C) instead of 192 KB + 64 KB.
+//               products A_mid W_hi + A_hi W_mid + A_hi W_hi into one accumulator; wgmma k16, 64 k-values per chunk.
+//               Error ~3 * 2^-18 per product (1e-5), far inside the 1e-3 budget of the path.
+// Both variants use the same weight tiles: a weight chunk is 128 rows x 128 B (32 tf32 or 64 bf16), 4 wgmma k-steps
+// of 32 bytes.
+//
+// Pre-split outputs for the window-attention kernels (lcab.cu), same 4 bytes per value: the consumer then needs no
+// conversion pass.  hi = bf16(x), mid = bf16(x - hi), packed bf16x2 with the lower channel in the low half.
+//   kind 1 (Q, K): channel pair (2j, 2j+1) -> words 2j = hi pair, 2j+1 = mid pair
+//   kind 2 (V):    channel group of 8      -> words 8g..8g+3 = hi pairs, 8g+4..8g+7 = mid pairs
+//   kind 3 (planar): group of 128 channels -> 64 hi words | 64 mid words
+// Every thread holds channel pairs (2j, 2j+1) of the accumulator, so each kind is a per-pair address computation.
+//
+// WRES: the whole [128, K<=128] weight slice (hi + lo, 128 KB) of this CTA's column tile stays resident in shared
+// memory (the grid is a multiple of n_tiles, so the column tile of a CTA never changes); only A streams.
 // ANCHW (convolution only): the input map is NCHW.  A TMA box must start on a 16-byte boundary in the innermost
-// dimension, so single-pixel tap shifts along x cannot be expressed as box coordinates of a channel-major map (probed:
-// tools/tma_nchw_probe.cu).  Instead ONE box [KE channels][8 rows][24 pixels] starting at x0 - 4 is loaded per (tap
-// row, channel chunk) into a 2-deep ring and serves the three taps of that row: the splitter reads column k of pixel
-// (y, x + 3 + dx) -- conflict-light LDS.32, lanes = pixels -- so no transposition pass is needed and the A traffic per
-// tap halves.  Weights stream through their own ring (one 32 KB hi|lo stage per tap and channel chunk).
+// dimension, so single-pixel tap shifts along x cannot be expressed as box coordinates of a channel-major map.
+// Instead ONE box [KE channels][8 rows][24 pixels] starting at x0 - 4 is loaded per (tap row, channel chunk) into a
+// 2-deep ring and serves the three taps of that row: the consumers read channel k of pixel (y, x + 3 + dx) straight
+// into their fragments.  Weights stream through their own ring (one 32 KB hi|lo stage per tap and channel chunk).
 template <bool WRES, bool BF, bool ANCHW>
 __global__ void __launch_bounds__(NTHREADS, 1)
 gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_constant__ CUtensorMap mapA1,
                   const __grid_constant__ CUtensorMap mapA2, const __grid_constant__ CUtensorMap mapWhi,
-                  const __grid_constant__ CUtensorMap mapWlo, const __grid_constant__ CUtensorMap mapC,
-                  const TcParams p) {
+                  const __grid_constant__ CUtensorMap mapWlo, const TcParams p) {
   extern __shared__ uint8_t smem_raw[];
   const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
-  uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
   constexpr int KE = BF ? 64 : 32;                                // k-values per chunk
   constexpr int AL = TM * KE * 4;                                 // fp32 A landing bytes per chunk (BF: two 16 KB boxes)
   static_assert(!(ANCHW && WRES), "the NCHW conv variant streams its weights");
   constexpr int AB = 24 * 8 * KE * 4;                             // ANCHW: bytes of one [KE][8][24] A box
-  constexpr int S = (BF && !WRES) ? 3 : 4;                        // pipeline stages
+  constexpr int S = WRES ? (BF ? 2 : 4) : (BF ? 3 : 4);           // pipeline stages
   constexpr int STG = ANCHW ? 2 * A_BYTES : (WRES ? AL : AL + 2 * A_BYTES);   // stage: [A landing |] W_hi | W_lo
   constexpr int NKW = BF ? 2 : 4;                                 // resident chunks (K <= 128)
   constexpr int WRES_BYTES = WRES ? 2 * NKW * A_BYTES : 0;        // resident W: hi chunks | lo chunks
   constexpr int RING_OFF = ANCHW ? 2 * AB : WRES_BYTES;           // stage ring starts after the resident weights / A ring
-  static_assert(RING_OFF + S * STG <= 192 * 1024, "operand ring exceeds its 192 KB");
-  constexpr int EP_OFF = RING_OFF + S * STG;
-  const uint32_t ep_base = base + EP_OFF;
-  const uint32_t bars = ep_base + EP_BYTES;
+  static_assert(RING_OFF + S * STG <= RING_BYTES, "operand ring exceeds its 192 KB");
+  constexpr int NCONS_WARPS = 8;
+  const uint32_t bars = base + RING_BYTES;
   auto full = [&](int s) { return bars + 8u * s; };
   auto empty = [&](int s) { return bars + 8u * (S + s); };
-  constexpr int NA = S;    // A_hi|A_lo buffers in tensor memory; NA == S: a_free(b) doubles as the stage-release barrier
-  // 3xTF32 is the PRECISE mode: the two small cross products accumulate in their own TMEM tile and are added to the
-  // main product in the epilogue.  The tensor core truncates at every accumulate, so the error of a tile grows with
-  // the number of instructions that hit its accumulator (measured ~K * 4e-8 with all three products in one tile);
-  // with the cross terms elsewhere the main tile sees K/8 instead of 3K/8 accumulations.  Accumulators are then
-  // single-buffered (TMEM: main 128 | cross 128 | 4 x 64 A), which costs the epilogue overlap -- acceptable, this
-  // mode only runs the decoder's index-/softmax-critical layers.
-  constexpr int NACC = BF ? 2 : 1;
-  constexpr uint32_t CROSS_COL = 128;                             // precise mode: cross-term accumulator columns
-  auto a_ready = [&](int b) { return bars + 8u * (2 * S + b); };
-  auto a_free = [&](int b) { return bars + 8u * (2 * S + NA + b); };
-  auto acc_full = [&](int a) { return bars + 8u * (2 * S + 2 * NA + a); };
-  auto acc_empty = [&](int a) { return bars + 8u * (2 * S + 2 * NA + 2 + a); };
-  const uint32_t tmem_slot = bars + 8u * (2 * S + 2 * NA + 4);
-  const uint32_t w_full = bars + 8u * (2 * S + 2 * NA + 5);
-  auto tq_full = [&](int i) { return bars + 8u * (2 * S + 2 * NA + 6 + i); };
-  auto tq_empty = [&](int i) { return bars + 8u * (2 * S + 2 * NA + 6 + V3_TQ + i); };
-  auto a2_full = [&](int i) { return bars + 8u * (2 * S + 2 * NA + 6 + 2 * V3_TQ + i); };       // ANCHW A-box ring
-  auto a2_empty = [&](int i) { return bars + 8u * (2 * S + 2 * NA + 6 + 2 * V3_TQ + 2 + i); };
-  static_assert(8 * (2 * S + 2 * NA + 6 + 2 * V3_TQ + 4) <= V3_BAR_BYTES, "barrier block overflow");
-  volatile int* tq = reinterpret_cast<volatile int*>(base_ptr + EP_OFF + EP_BYTES + V3_BAR_BYTES + 512);
-  volatile uint32_t* tmem_slot_ptr =
-      reinterpret_cast<volatile uint32_t*>(base_ptr + EP_OFF + EP_BYTES + 8 * (2 * S + 2 * NA + 4));
+  const uint32_t w_full = bars + 8u * (2 * S);
+  auto a2_full = [&](int i) { return bars + 8u * (2 * S + 1 + i); };       // ANCHW A-box ring
+  auto a2_empty = [&](int i) { return bars + 8u * (2 * S + 3 + i); };
+  static_assert(8 * (2 * S + 5) <= BAR_BYTES, "barrier block overflow");
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (threadIdx.x == 0) DBG_STAMP(7, 100);            // kernel entry
-  if (warp == 2 && lane < 6) {                         // pull the six TMA descriptors into the descriptor cache early
-    const CUtensorMap* mp = lane == 0 ? &mapA0 : lane == 1 ? &mapA1 : lane == 2 ? &mapA2 : lane == 3 ? &mapWhi
-                            : lane == 4 ? &mapWlo : &mapC;
+  if (warp == 1 && lane < 5) {                         // pull the TMA descriptors into the descriptor cache early
+    const CUtensorMap* mp = lane == 0 ? &mapA0 : lane == 1 ? &mapA1 : lane == 2 ? &mapA2 : lane == 3 ? &mapWhi : &mapWlo;
     asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(mp)) : "memory");
   }
   int nk = 0;
@@ -253,36 +127,16 @@ gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(full(s), 1);
-      mbar_init(empty(s), WRES ? 4 : 1);            // WRES: the splitter frees the A landing buffer
+      mbar_init(empty(s), NCONS_WARPS);
     }
     mbar_init(w_full, 1);
-    for (int b = 0; b < NA; ++b) {
-      mbar_init(a_ready(b), 4);
-      mbar_init(a_free(b), 1);
-    }
-    for (int b = 0; b < 2; ++b) {
-      mbar_init(acc_full(b), 1);
-      mbar_init(acc_empty(b), 4);
-    }
-    for (int i = 0; i < V3_TQ; ++i) {
-      mbar_init(tq_full(i), 1);
-      mbar_init(tq_empty(i), 9);                     // MMA warp + 4 splitter warps + 4 epilogue warps
-    }
     for (int i = 0; i < 2; ++i) {
       mbar_init(a2_full(i), 1);
-      mbar_init(a2_empty(i), 4);                     // the four splitter warps
+      mbar_init(a2_empty(i), NCONS_WARPS);
     }
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
   }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-  if (threadIdx.x == 0) DBG_STAMP(7, 101);            // barriers + TMEM ready
 
   auto tile_coords = [&](int tile, int& m0, int& n0, int& img, int& y0, int& x0) {
     const int mt = tile / p.n_tiles, nt = tile - mt * p.n_tiles;
@@ -298,56 +152,22 @@ gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_consta
     }
   };
 
-  // Tiles are handed out by global atomic counters (one per column tile when the weights are resident), NOT by a
-  // static blockIdx stride: when some of the grid's CTAs cannot become resident (another stream holds a few SMs)
-  // the resident CTAs simply take more tiles, instead of the late CTAs running their whole share afterwards.
-  // Warp 0 fetches ids ahead of time and publishes them through a small shared-memory queue.
-  auto take_tile = [&](int tl) -> int {               // consumer side: id of this CTA's tl-th tile, or -1
-    const int i = tl % V3_TQ;
-    mbar_wait(tq_full(i), (tl / V3_TQ) & 1);
-    const int tile = tq[i];
-    __syncwarp();
-    if (lane == 0) mbar_arrive(tq_empty(i));
-    return tile;
-  };
-
-  if (warp == 0) {
+  if (warp < 4) {
     // ---------------- TMA producer ----------------
-    if (lane == 0) {
+    // one thread issues all loads: the warpgroup hands most of its registers to the consumers (128 x 40 + 256 x 232)
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
       int it = 0, t3 = 0;
-      const int group = WRES ? (int)(blockIdx.x % p.n_tiles) : 0;
-      int published = 0;
-      bool exhausted = false;
-      auto publish = [&]() {                          // fetch one more tile id, L2-prefetch its A rows, queue it
-        const int i = published % V3_TQ;
-        if (published >= V3_TQ) mbar_wait(tq_empty(i), ((published / V3_TQ) - 1) & 1);
-        int tile;
-        if (WRES) {
-          const int mt = atomicAdd(p.sched + group, 1);
-          tile = mt < p.m_tiles ? mt * p.n_tiles + group : -1;
-        } else {
-          tile = atomicAdd(p.sched, 1);
-          if (tile >= num_tiles) tile = -1;
+      if (WRES && (int)blockIdx.x < num_tiles) {
+        // resident weights: gridDim.x % n_tiles == 0, so the column tile of this CTA is fixed
+        const int n0w = (int)(blockIdx.x % p.n_tiles) * TN;
+        mbar_expect_tx(w_full, 2 * nk * A_BYTES);
+        for (int kc = 0; kc < nk; ++kc) {
+          tma_load_2d(base + kc * A_BYTES, &mapWhi, w_full, kc * KE, n0w);
+          tma_load_2d(base + (NKW + kc) * A_BYTES, &mapWlo, w_full, kc * KE, n0w);
         }
-        if (tile >= 0 && !p.conv) {
-          const int mt = tile / p.n_tiles;
-          for (int src = 0; src < p.nsrc; ++src)
-              for (int kc = 0; kc < tc_kch(p, src); ++kc) {
-                const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
-                tma_prefetch_2d(mp, kc * KE, mt * TM);
-                if (BF) tma_prefetch_2d(mp, kc * KE + 32, mt * TM);
-              }
-        }
-        tq[i] = tile;
-        mbar_arrive(tq_full(i));
-        exhausted = tile < 0;
-        ++published;
-      };
-      constexpr int PF = 2;                           // tile ids (and their L2 prefetch) run this far ahead
-      publish();
-      for (int n = 0;; ++n) {
-        const int tile = tq[n % V3_TQ];
-        if (tile < 0) break;
+      }
+      for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
         int m0, n0, img, y0, x0;
         tile_coords(tile, m0, n0, img, y0, x0);
         if (ANCHW) {
@@ -359,7 +179,7 @@ gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_consta
               tma_load_4d(base + ab * AB, &mapA0, a2_full(ab), x0 - 4, y0 + dy - 1, kc * KE, img);
               for (int dx = 0; dx < 3; ++dx, ++it) {
                 const int s = it % S;
-                if (it >= S) mbar_wait(a_free(s), ((it / S) - 1) & 1);
+                if (it >= S) mbar_wait(empty(s), ((it / S) - 1) & 1);
                 DBG_STAMP(0, it);
                 const uint32_t st = base + RING_OFF + s * STG;
                 const int kw = ((dy * 3 + dx) * p.k0 + kc) * KE;
@@ -368,347 +188,221 @@ gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_consta
                 tma_load_2d(st + A_BYTES, &mapWlo, full(s), kw, n0);
               }
             }
-        } else
-        for (int kc_all = 0; kc_all < nk; ++kc_all, ++it) {
-          const int s = it % S;
-          if (it >= S) mbar_wait(WRES ? empty(s) : a_free(s), ((it / S) - 1) & 1);
-          DBG_STAMP(0, it);
-          const uint32_t st = base + RING_OFF + s * STG;
-          mbar_expect_tx(full(s), STG);
-          if (p.conv) {
-            const int tap = kc_all / p.k0, kc = kc_all - tap * p.k0;
-            tma_load_4d(st, &mapA0, full(s), kc * KE, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
-            if (BF) tma_load_4d(st + A_BYTES, &mapA0, full(s), kc * KE + 32, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
-          } else {
-            int src = 0, kc = kc_all;
-            while (kc >= tc_kch(p, src)) {
-              kc -= tc_kch(p, src);
-              ++src;
-            }
-            const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
-            tma_load_2d(st, mp, full(s), kc * KE, m0);
-            if (BF) tma_load_2d(st + A_BYTES, mp, full(s), kc * KE + 32, m0);
-          }
-          if (!WRES) {
-            tma_load_2d(st + AL, &mapWhi, full(s), kc_all * KE, n0);
-            tma_load_2d(st + AL + A_BYTES, &mapWlo, full(s), kc_all * KE, n0);
-          }
-        }
-        if (WRES && n == 0) {
-          // resident weights (gridDim.x % n_tiles == 0 => the column tile of this CTA is fixed).  Issued AFTER the
-          // first tile's A chunks: the splitter needs A first, and 148 CTAs pulling the same 128 KB at once is
-          // the slowest part of the start-up.
-          const int n0w = group * TN;
-          mbar_expect_tx(w_full, 2 * nk * A_BYTES);
-          for (int kc = 0; kc < nk; ++kc) {
-            tma_load_2d(base + kc * A_BYTES, &mapWhi, w_full, kc * KE, n0w);
-            tma_load_2d(base + (NKW + kc) * A_BYTES, &mapWlo, w_full, kc * KE, n0w);
-          }
-        }
-        while (!exhausted && published <= n + 1 + PF) publish();   // ids (atomics) + L2 prefetch run ahead of the loads
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer: A from TMEM, W from shared memory ----------------
-    // The whole warp runs the (uniform) control flow; the tcgen05 instructions sit under an elect.sync predicate.
-    // (Under a plain `lane == 0` branch ptxas wraps every UTCMMA in an ELECT / BRA.U.ANY loop over the active
-    // lanes, ~45 cycles per instruction: the issue thread, not the tensor pipe, then sets the pace.)
-    int it = 0;
-    for (int tl = 0;; ++tl) {
-      const int tile = take_tile(tl);
-      if (tile < 0) break;
-      if (WRES && tl == 0) mbar_wait(w_full, 0);
-      // MMA width = the valid columns of this tile rounded up to 16: a 10-class heat-map conv issues N = 16
-      // instructions (8 cycles) instead of N = 128 (64 cycles) and reads 1/8 of the weight tile
-      const int ncols = min(TN, p.N - (tile % p.n_tiles) * TN);
-      const uint32_t idesc = ((BF ? IDESC_BF16 : IDESC) & ~(0x3Fu << 17)) | ((uint32_t)(((ncols + 15) & ~15) >> 3) << 17);
-      const int a = tl % NACC;
-      if (tl >= NACC) mbar_wait(acc_empty(a), ((tl / NACC) - 1) & 1);
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(a * TN);
-      for (int kc_all = 0; kc_all < nk; ++kc_all, ++it) {
-        const int s = it % S, b = it % NA;
-        mbar_wait(a_ready(b), (it / NA) & 1);       // A_hi/A_lo of this chunk are in TMEM (implies full[s])
-        if (ANCHW) mbar_wait(full(s), (it / S) & 1);    // ... except here: the weights land on their own barrier
-        tc_fence_after();
-        const uint32_t st = base + RING_OFF + s * STG;
-        const uint32_t whi_base = ANCHW ? st : (WRES ? base + kc_all * A_BYTES : st + AL);
-        const uint32_t wlo_base = ANCHW ? st + A_BYTES : (WRES ? base + (NKW + kc_all) * A_BYTES : st + AL + A_BYTES);
-        const uint32_t ta = tmem_base + 256u + (uint32_t)(b * 64);
-        if (elect_one()) {
-          DBG_STAMP(3, it);
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {               // 4 k-steps of 32 operand bytes: 8 tf32 or 16 bf16 each
-            const uint64_t w_hi = umma_desc(whi_base + k * 32), w_lo = umma_desc(wlo_base + k * 32);
-            if (BF) {
-              umma_bf16_ts(tmem_acc, ta + 32u + (uint32_t)(k * 8), w_hi, idesc, (kc_all | k) != 0);  // A_mid * W_hi
-              umma_bf16_ts(tmem_acc, ta + (uint32_t)(k * 8), w_lo, idesc, 1);                         // A_hi * W_mid
-              umma_bf16_ts(tmem_acc, ta + (uint32_t)(k * 8), w_hi, idesc, 1);                         // A_hi * W_hi
+        } else {
+          for (int kc_all = 0; kc_all < nk; ++kc_all, ++it) {
+            const int s = it % S;
+            if (it >= S) mbar_wait(empty(s), ((it / S) - 1) & 1);
+            DBG_STAMP(0, it);
+            const uint32_t st = base + RING_OFF + s * STG;
+            mbar_expect_tx(full(s), STG);
+            if (p.conv) {
+              const int tap = kc_all / p.k0, kc = kc_all - tap * p.k0;
+              tma_load_4d(st, &mapA0, full(s), kc * KE, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
+              if (BF) tma_load_4d(st + A_BYTES, &mapA0, full(s), kc * KE + 32, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
             } else {
-              umma_tf32_ts(tmem_acc + CROSS_COL, ta + 32u + (uint32_t)(k * 8), w_hi, idesc, (kc_all | k) != 0);  // A_lo * W_hi
-              umma_tf32_ts(tmem_acc + CROSS_COL, ta + (uint32_t)(k * 8), w_lo, idesc, 1);                         // A_hi * W_lo
-              umma_tf32_ts(tmem_acc, ta + (uint32_t)(k * 8), w_hi, idesc, (kc_all | k) != 0);                     // A_hi * W_hi
+              int src = 0, kc = kc_all;
+              while (kc >= tc_kch(p, src)) {
+                kc -= tc_kch(p, src);
+                ++src;
+              }
+              const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
+              tma_load_2d(st, mp, full(s), kc * KE, m0);
+              if (BF) tma_load_2d(st + A_BYTES, mp, full(s), kc * KE + 32, m0);
+            }
+            if (!WRES) {
+              tma_load_2d(st + AL, &mapWhi, full(s), kc_all * KE, n0);
+              tma_load_2d(st + AL + A_BYTES, &mapWlo, full(s), kc_all * KE, n0);
             }
           }
-          // one commit per chunk: a_free(b) releases the TMEM A buffer to the splitter AND (streamed weights,
-          // NA == S so b == s) the shared-memory stage to the TMA producer
-          umma_commit(a_free(b));
-          if (kc_all == nk - 1) umma_commit(acc_full(a));
-          DBG_STAMP(4, it);
-        }
-        __syncwarp();
-      }
-    }
-  } else if (warp < 6) {
-    // ---------------- splitter (warps 2..5): smem A chunk -> registers -> hi/lo -> TMEM ----------------
-    const int qd = warp & 3;                          // TMEM lane quarter of this warp
-    const int row = qd * 32 + lane;
-    int it = 0;
-    for (int tl = 0;; ++tl) {
-      if (take_tile(tl) < 0) break;
-      for (int kc_all = 0; kc_all < nk; ++kc_all, ++it) {
-        const int s = it % S, b = it % NA;
-        uint32_t hi[32], lo[32];
-        if (ANCHW) {
-          const int t3 = it / 3, dx = it - 3 * t3, ab = t3 & 1;
-          if (dx == 0) mbar_wait(a2_full(ab), (t3 >> 1) & 1);
-          if (threadIdx.x == 64) DBG_STAMP(1, it);
-          // box [KE][8][24]: channel k of pixel (y, x) shifted by the tap = float k * 192 + y * 24 + x + 3 + dx
-          const float* acol = reinterpret_cast<const float*>(base_ptr + ab * AB) + ((row >> 4) * 24 + (row & 15) + 3 + dx);
-          if (BF) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float a0 = acol[(2 * j) * 192], a1 = acol[(2 * j + 1) * 192];
-              const uint32_t h = pack_bf16x2(a0, a1);
-              hi[j] = h;
-              lo[j] = pack_bf16x2(a0 - __uint_as_float(h << 16), a1 - __uint_as_float(h & 0xFFFF0000u));
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) {
-              const float a0 = acol[j * 192];
-              hi[j] = (__float_as_uint(a0) + 0x1000u) & 0xFFFFE000u;
-              lo[j] = __float_as_uint(a0 - __uint_as_float(hi[j]));
-            }
-          }
-          if (dx == 2) {                               // last tap of this box: hand the buffer back
-            __syncwarp();
-            if (lane == 0) mbar_arrive(a2_empty(ab));
-          }
-        } else {
-        mbar_wait(full(s), (it / S) & 1);
-        if (threadIdx.x == 64) DBG_STAMP(1, it);
-        const uint8_t* arow = base_ptr + RING_OFF + s * STG + row * 128;
-        if (BF) {
-          // 64 k-values (two 128 B rows) -> 32 packed bf16x2 hi + 32 packed mid; column c holds k = 2c, 2c + 1
-#pragma unroll
-          for (int h = 0; h < 2; ++h)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float4 x = *reinterpret_cast<const float4*>(arow + h * A_BYTES + ((j ^ (row & 7)) << 4));
-              const uint32_t h01 = pack_bf16x2(x.x, x.y), h23 = pack_bf16x2(x.z, x.w);
-              hi[h * 16 + 2 * j] = h01;
-              hi[h * 16 + 2 * j + 1] = h23;
-              lo[h * 16 + 2 * j] = pack_bf16x2(x.x - __uint_as_float(h01 << 16), x.y - __uint_as_float(h01 & 0xFFFF0000u));
-              lo[h * 16 + 2 * j + 1] = pack_bf16x2(x.z - __uint_as_float(h23 << 16), x.w - __uint_as_float(h23 & 0xFFFF0000u));
-            }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 x = *reinterpret_cast<const float4*>(arow + ((j ^ (row & 7)) << 4));   // undo the 128B swizzle
-            const float xv[4] = {x.x, x.y, x.z, x.w};
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              hi[4 * j + e] = (__float_as_uint(xv[e]) + 0x1000u) & 0xFFFFE000u;        // round to nearest tf32
-              lo[4 * j + e] = __float_as_uint(xv[e] - __uint_as_float(hi[4 * j + e]));   // exact remainder
-            }
+          const int nxt = tile + (int)gridDim.x;       // L2 prefetch of the next tile's A rows
+          if (nxt < num_tiles && !p.conv) {
+            const int mt = nxt / p.n_tiles;
+            for (int src = 0; src < p.nsrc; ++src)
+              for (int kc = 0; kc < tc_kch(p, src); ++kc) {
+                const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
+                tma_prefetch_2d(mp, kc * KE, mt * TM);
+                if (BF) tma_prefetch_2d(mp, kc * KE + 32, mt * TM);
+              }
           }
         }
-        }   // !ANCHW
-        if (WRES) {                                   // the landing buffer is free as soon as every lane has read it
-          __syncwarp();
-          if (lane == 0) mbar_arrive(empty(s));
-        }
-        if (it >= NA) mbar_wait(a_free(b), ((it / NA) - 1) & 1);  // MMAs that read this TMEM A buffer retired
-        tc_fence_after();
-        const uint32_t ta = tmem_base + ((uint32_t)(qd * 32) << 16) + 256u + (uint32_t)(b * 64);
-        tmem_st32(ta, hi);
-        tmem_st32(ta + 32u, lo);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_ready(b));
-        if (threadIdx.x == 64) DBG_STAMP(2, it);
       }
     }
   } else {
-    // ---------------- epilogue (warps 6..9): TMEM -> registers -> swizzled smem -> TMA store ----------------
-    // Per tile a warp owns 32 accumulator rows.  It reads them 64 columns at a time (two tcgen05.ld in flight),
-    // applies bias / residual / activation in registers, stages each 32x32 block in a 128B-swizzled 4 KB buffer and
-    // hands it to the TMA store engine (which also clips the M / N edges).  Two staging buffers per warp:
-    // cp.async.bulk.wait_group.read 1 before a buffer is rewritten.  The accumulator is released to the MMA warp
-    // as soon as the last tcgen05.ld of the tile has completed, i.e. before the stores of that tile are issued.
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t my_ep = ep_base + (uint32_t)((warp - 6) * 2) * 4096u;
-    float* bias_s = reinterpret_cast<float*>(base_ptr + EP_OFF + EP_BYTES + V3_BAR_BYTES);
-    int tl = 0, chunk = 0, bias_n0 = -1;
-    for (;; ++tl) {
-      const int tile = take_tile(tl);
-      if (tile < 0) break;
+    // ---------------- consumers (warpgroups 1, 2): 64 rows each ----------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = wg * 64 + wl * 16 + g, r1 = r0 + 8;   // tile rows of this thread's fragments
+    constexpr int NX = BF ? 1 : 64;
+    float acc[64], accx[NX];
+    int it = 0;
+    bool w_ready = !WRES;
+    for (int tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
       int m0, n0, img, y0, x0;
       tile_coords(tile, m0, n0, img, y0, x0);
-      if (n0 != bias_n0) {
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        const int c = n0 + (int)threadIdx.x - 192;
-        bias_s[threadIdx.x - 192] = (p.bias && c < p.N) ? __ldg(p.bias + c) : 0.f;
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        bias_n0 = n0;
+      if (!w_ready) {
+        mbar_wait(w_full, 0);
+        w_ready = true;
       }
-      const int a = tl % NACC;
-      mbar_wait(acc_full(a), (tl / NACC) & 1);
-      tc_fence_after();
-      if (threadIdx.x == 192) DBG_STAMP(5, tl);
-      long long grow;
-      if (p.conv) {
-        const int yy = min(y0 + row / 16, p.H - 1), xx = min(x0 + row % 16, p.W - 1);
-        grow = ((long long)img * p.H + yy) * p.W + xx;
-      } else {
-        grow = min((long long)(m0 + row), (long long)p.M - 1);
-      }
-      const float* resrow = p.res ? p.res + (size_t)(grow % p.res_mod) * p.ldres : nullptr;
-      const int act = p.act;
-      const int ncols = min(TN, p.N - n0);                       // valid columns of this tile (multiple of 4)
-
-      auto prep_block = [&](float (&v)[32], int c0) {            // bias / residual / activation in registers
-        const int col = n0 + c0;
-        const bool fullc = c0 + 32 <= ncols;
-#pragma unroll
-        for (int j = 0; j < 8; ++j) {
-          const float4 b4 = *reinterpret_cast<const float4*>(bias_s + c0 + 4 * j);      // broadcast LDS
-          v[4 * j] += b4.x; v[4 * j + 1] += b4.y; v[4 * j + 2] += b4.z; v[4 * j + 3] += b4.w;
+      for (int kc_all = 0; kc_all < nk; ++kc_all, ++it) {
+        const int s = it % S;
+        const uint32_t st = base + RING_OFF + s * STG;
+        mbar_wait(full(s), (it / S) & 1);
+        if (threadIdx.x == 128) DBG_STAMP(1, it);
+        // A element (row, k) of this chunk -> shared-memory address
+        int t3 = 0, dx = 0, ab = 0;
+        if (ANCHW) {
+          t3 = it / 3; dx = it - 3 * t3; ab = t3 & 1;
+          if (dx == 0) mbar_wait(a2_full(ab), (t3 >> 1) & 1);
         }
-        if (resrow) {
-          if (fullc) {
-            float4 r4[8];
+        const float* abox = reinterpret_cast<const float*>(base_ptr + (ANCHW ? ab * AB : RING_OFF + s * STG));
+        auto a_at = [&](int row, int k) -> float {      // k < KE
+          if (ANCHW) return abox[k * 192 + (row >> 4) * 24 + (row & 15) + 3 + dx];
+          const int h = k >> 5, kk = k & 31;           // BF: two 32-column boxes
+          return abox[h * (A_BYTES / 4) + row * 32 + ((((kk >> 2) ^ (row & 7))) << 2) + (kk & 3)];
+        };
+        auto a_pair = [&](int row, int k) -> float2 {   // (k, k + 1), k even
+          if (ANCHW) return make_float2(a_at(row, k), a_at(row, k + 1));
+          const int h = k >> 5, kk = k & 31;
+          return *reinterpret_cast<const float2*>(abox + h * (A_BYTES / 4) + row * 32 + ((((kk >> 2) ^ (row & 7))) << 2) +
+                                                  (kk & 3));
+        };
+        const uint32_t whi = WRES ? base + kc_all * A_BYTES : st + (ANCHW ? 0 : AL);
+        const uint32_t wlo = WRES ? base + (NKW + kc_all) * A_BYTES : st + (ANCHW ? 0 : AL) + A_BYTES;
 #pragma unroll
-            for (int j = 0; j < 8; ++j) r4[j] = ldg4(resrow + col + 4 * j);
+        for (int hf = 0; hf < 2; ++hf) {                // two k-steps per wgmma group
+          uint32_t ahi[2][4], alo[2][4];
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              v[4 * j] += r4[j].x; v[4 * j + 1] += r4[j].y; v[4 * j + 2] += r4[j].z; v[4 * j + 3] += r4[j].w;
+          for (int u = 0; u < 2; ++u) {
+            const int ks = 2 * hf + u;
+            if (BF) {
+              const int kb = 16 * ks + 2 * t;
+              const float2 x[4] = {a_pair(r0, kb), a_pair(r1, kb), a_pair(r0, kb + 8), a_pair(r1, kb + 8)};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                const uint32_t h = pack_bf16x2(x[e].x, x[e].y);
+                ahi[u][e] = h;
+                alo[u][e] = pack_bf16x2(x[e].x - __uint_as_float(h << 16), x[e].y - __uint_as_float(h & 0xFFFF0000u));
+              }
+            } else {
+              const int kb = 8 * ks + t;
+              const float x[4] = {a_at(r0, kb), a_at(r1, kb), a_at(r0, kb + 4), a_at(r1, kb + 4)};
+#pragma unroll
+              for (int e = 0; e < 4; ++e) {
+                ahi[u][e] = (__float_as_uint(x[e]) + 0x1000u) & 0xFFFFE000u;        // round to nearest tf32
+                alo[u][e] = __float_as_uint(x[e] - __uint_as_float(ahi[u][e]));     // exact remainder
+              }
             }
-          } else {
+          }
+          fence_regs(acc);
+          if (!BF) fence_regs(accx);
+          wgmma_fence();
 #pragma unroll
-            for (int j = 0; j < 32; ++j)
-              if (c0 + j < ncols) v[j] += __ldg(resrow + col + j);
+          for (int u = 0; u < 2; ++u) {
+            const int ks = 2 * hf + u;
+            const uint32_t first = (kc_all | ks) != 0;
+            const uint64_t w_hi = wgmma_desc(whi + ks * 32), w_lo = wgmma_desc(wlo + ks * 32);
+            if constexpr (BF) {
+              wgmma_bf16_rs(acc, alo[u], w_hi, first);   // A_mid * W_hi
+              wgmma_bf16_rs(acc, ahi[u], w_lo, 1);       // A_hi * W_mid
+              wgmma_bf16_rs(acc, ahi[u], w_hi, 1);       // A_hi * W_hi
+            } else {
+              wgmma_tf32_rs(accx, alo[u], w_hi, first);  // A_lo * W_hi
+              wgmma_tf32_rs(accx, ahi[u], w_lo, 1);      // A_hi * W_lo
+              wgmma_tf32_rs(acc, ahi[u], w_hi, first);   // A_hi * W_hi
+            }
+          }
+          wgmma_commit();
+          wgmma_wait_all();
+          fence_regs(acc);
+          if (!BF) fence_regs(accx);
+        }
+        if (threadIdx.x == 128) DBG_STAMP(4, it);
+        __syncwarp();
+        if (lane == 0) {
+          mbar_arrive(empty(s));                        // stage (A landing and / or weights) read by this warp
+          if (ANCHW && dx == 2) mbar_arrive(a2_empty(ab));
+        }
+      }
+      if constexpr (!BF) {
+#pragma unroll
+        for (int j = 0; j < 64; ++j) acc[j] += accx[j];
+      }
+      // ---------------- epilogue: bias / residual / activation, stores ----------------
+      long long grow[2];
+      bool rok[2];
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = h ? r1 : r0;
+        if (p.conv) {
+          const int yy = y0 + row / 16, xx = x0 + row % 16;
+          rok[h] = yy < p.H && xx < p.W;
+          grow[h] = ((long long)img * p.H + min(yy, p.H - 1)) * p.W + min(xx, p.W - 1);
+        } else {
+          rok[h] = m0 + row < p.M;
+          grow[h] = min((long long)(m0 + row), (long long)p.M - 1);
+        }
+      }
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = n0 + 8 * j + 2 * t;
+        if (col < p.N) {                                // N % 4 == 0: the pair is valid as a whole
+          float2 b2 = make_float2(0.f, 0.f);
+          if (p.bias) b2 = *reinterpret_cast<const float2*>(p.bias + col);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            acc[4 * j + 2 * h] += b2.x;
+            acc[4 * j + 2 * h + 1] += b2.y;
+            if (p.res) {
+              const float2 r2 = *reinterpret_cast<const float2*>(p.res + (size_t)(grow[h] % p.res_mod) * p.ldres + col);
+              acc[4 * j + 2 * h] += r2.x;
+              acc[4 * j + 2 * h + 1] += r2.y;
+            }
           }
         }
-        act_tile(v, act);
-      };
-      auto store_block = [&](float (&v)[32], int col) {          // 32 words per row -> staging -> TMA store at word column col
-        const uint32_t buf = my_ep + (uint32_t)(chunk & 1) * 4096u;
-        if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");   // buffer's previous store done
-        __syncwarp();
+      }
+      if (p.act == DI_ACT_RELU) {                       // one warp-uniform branch per activation (no per-element
+#pragma unroll                                          // if-conversion of the GELU polynomial)
+        for (int j = 0; j < 64; ++j) acc[j] = fmaxf(acc[j], 0.f);
+      } else if (p.act == DI_ACT_GELU) {
 #pragma unroll
-        for (int j = 0; j < 8; ++j)
-          asm volatile("st.shared.v4.f32 [%0], {%1, %2, %3, %4};" ::"r"(buf + lane * 128 + ((j ^ (lane & 7)) << 4)),
-                       "f"(v[4 * j]), "f"(v[4 * j + 1]), "f"(v[4 * j + 2]), "f"(v[4 * j + 3])
-                       : "memory");
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        __syncwarp();
-        if (lane == 0 && !(p.dbg & 4)) {
-          if (p.conv) tma_store_4d(&mapC, buf, col, x0, y0 + 2 * q, img);
-          else tma_store_2d(&mapC, buf, col, m0 + 32 * q);
-          asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-        }
-        ++chunk;
-      };
-      auto finish_block = [&](float (&v)[32], int c0) {          // bias/res/act -> staging -> TMA store
-        const int col = n0 + c0;
-        prep_block(v, c0);
-        if (p.split_kind && col >= p.split_col0) split_block(v, p.split_kind);
-        store_block(v, col);
-      };
-      // split kind 3 ("planar", the operand format of the tcgen05 window kernel, lcab_tc.cu): every group of 128
-      // output channels becomes 64 words of bf16 hi followed by 64 words of bf16 mid; one call handles 64 channels
-      // (v0 = channels c0..c0+31, v1 = c0+32..c0+63) = 32 hi words + 32 mid words.
-      auto finish_pair_planar = [&](float (&v0)[32], float (&v1)[32], int c0) {
-        prep_block(v0, c0);
-        prep_block(v1, c0 + 32);
-        uint32_t h[32], m[32];
+        for (int j = 0; j < 64; ++j) acc[j] = 0.5f * acc[j] * (1.f + erff(acc[j] * 0.70710678118654752440f));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        if (!rok[h]) continue;
+        float* crow = p.C + (size_t)grow[h] * p.ldc;
 #pragma unroll
         for (int j = 0; j < 16; ++j) {
-          h[j] = pack_bf16x2(v0[2 * j], v0[2 * j + 1]);
-          m[j] = pack_bf16x2(v0[2 * j] - __uint_as_float(h[j] << 16), v0[2 * j + 1] - __uint_as_float(h[j] & 0xFFFF0000u));
-          h[16 + j] = pack_bf16x2(v1[2 * j], v1[2 * j + 1]);
-          m[16 + j] = pack_bf16x2(v1[2 * j] - __uint_as_float(h[16 + j] << 16), v1[2 * j + 1] - __uint_as_float(h[16 + j] & 0xFFFF0000u));
-        }
-#pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          v0[j] = __uint_as_float(h[j]);
-          v1[j] = __uint_as_float(m[j]);
-        }
-        const int rel = n0 + c0 - p.split_col0;
-        const int wcol = p.split_col0 + (rel & ~127) + ((rel & 127) >> 1);
-        store_block(v0, wcol);
-        store_block(v1, wcol + 64);
-      };
-
-      const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(a * TN);
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        const int c0 = h * 64;
-        if (c0 >= ncols) break;
-        const bool two = c0 + 32 < ncols;
-        float v0[32], v1[32];
-        tmem_ld32_nowait(tacc + (uint32_t)c0, v0);
-        if (two) tmem_ld32_nowait(tacc + (uint32_t)(c0 + 32), v1);
-        if (!BF) {                                               // precise mode: add the cross-term tile
-          float x[32];
-          tmem_ld32_nowait(tacc + CROSS_COL + (uint32_t)c0, x);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int j = 0; j < 32; ++j) v0[j] += x[j];
-          if (two) {
-            tmem_ld32_nowait(tacc + CROSS_COL + (uint32_t)(c0 + 32), x);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 32; ++j) v1[j] += x[j];
+          const int col = n0 + 8 * j + 2 * t;
+          if (col >= p.N) continue;
+          const float v0 = acc[4 * j + 2 * h], v1 = acc[4 * j + 2 * h + 1];
+          if (p.split_kind && col >= p.split_col0) {
+            const uint32_t hi = pack_bf16x2(v0, v1);
+            const uint32_t mid = pack_bf16x2(v0 - __uint_as_float(hi << 16), v1 - __uint_as_float(hi & 0xFFFF0000u));
+            uint32_t* cw = reinterpret_cast<uint32_t*>(crow);
+            if (p.split_kind == 1) {
+              *reinterpret_cast<uint2*>(cw + col) = make_uint2(hi, mid);
+            } else if (p.split_kind == 2) {
+              const int g8 = col & ~7, q = (col & 7) >> 1;
+              cw[g8 + q] = hi;
+              cw[g8 + 4 + q] = mid;
+            } else {
+              const int rel = col - p.split_col0;
+              const int w0 = p.split_col0 + (rel & ~127) + ((rel & 127) >> 1);
+              cw[w0] = hi;
+              cw[w0 + 64] = mid;
+            }
+          } else {
+            *reinterpret_cast<float2*>(crow + col) = make_float2(v0, v1);
           }
         }
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (h == 1 || c0 + 64 >= ncols) {                        // last TMEM read of this tile: release the accumulator
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(acc_empty(a));
-        }
-        if (threadIdx.x == 192) DBG_STAMP(7, (tl * 2 + h) * 3 + 0);
-        if (p.split_kind == 3 && n0 + c0 >= p.split_col0) {
-          finish_pair_planar(v0, v1, c0);
-        } else {
-          finish_block(v0, c0);
-          if (threadIdx.x == 192) DBG_STAMP(7, (tl * 2 + h) * 3 + 1);
-          if (two) finish_block(v1, c0 + 32);
-        }
-        if (threadIdx.x == 192) DBG_STAMP(7, (tl * 2 + h) * 3 + 2);
       }
-      if (threadIdx.x == 192) DBG_STAMP(6, tl);
+      if (threadIdx.x == 128) DBG_STAMP(6, (tile - (int)blockIdx.x) / (int)gridDim.x);
     }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");   // all stores retired before exit
   }
-  tc_fence_before();
   __syncthreads();
   if (threadIdx.x == 0) DBG_STAMP(7, 102);            // all roles done
-  if (threadIdx.x == 0) {                              // the last CTA to finish re-arms the scheduler slot
-    __threadfence();
-    if (atomicAdd(p.sched + 15, 1) == (int)gridDim.x - 1) {
-      for (int i = 0; i < 16; ++i) p.sched[i] = 0;
-      __threadfence();
-    }
-  }
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
 }
 
 // ---- host side ----------------------------------------------------------------------------------
@@ -765,30 +459,7 @@ bool make_map_nchw(CUtensorMap* m, const float* ptr, int N, int H, int W, int C,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
-// store maps: 2-D [rows, cols] box 32 x 32, or 4-D NHWC box 32 ch x 16 x 2 x 1 (one epilogue warp's rows)
-bool make_store_map_2d(CUtensorMap* m, float* ptr, long long rows, long long cols, long long ld) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * 4};
-  cuuint32_t box[2] = {32, 32};
-  cuuint32_t estr[2] = {1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-bool make_store_map_nhwc(CUtensorMap* m, float* ptr, int N, int H, int W, int C) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
-  cuuint32_t box[4] = {32, 16, 2, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, ptr, dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-// Per-device launch state (one process may drive several GPUs): SM count, the one-time shared-memory attribute and
-// the address of this device's copy of the scheduler pool.
+// Per-device launch state (one process may drive several GPUs): SM count and the one-time shared-memory attribute.
 constexpr int MAX_DEV = 64;
 struct DevState {
   int num_sms = 0;
@@ -800,13 +471,12 @@ int g_tc_wres = 1;    // keep the weight slice resident in shared memory when K 
 int g_tc_sm_limit = 0; // > 0: persistent grids use at most this many CTAs (leaves SMs to kernels of other streams)
 
 template <bool WRES, bool BF, bool ANCHW = false>
-void launch_v3(dim3 grid, const CUtensorMap maps[6], const TcParams& p, cudaStream_t stream) {
-  gemm_tc_kernel_v3<WRES, BF, ANCHW><<<grid, NTHREADS, V3_SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4], maps[5], p);
+void launch_v3(dim3 grid, const CUtensorMap maps[5], const TcParams& p, cudaStream_t stream) {
+  gemm_tc_kernel_v3<WRES, BF, ANCHW><<<grid, NTHREADS, V3_SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4], p);
 }
 
 // bf = 1: bf16-split operands (chunks of 64 k-values), 0: 3xTF32 (chunks of 32)
-int launch_tc(const CUtensorMap maps[6], const TcParams& p_in, int bf, cudaStream_t stream, const char* name) {
-  TcParams p = p_in;
+int launch_tc(const CUtensorMap maps[5], const TcParams& p, int bf, cudaStream_t stream, const char* name) {
   int devid = 0;
   cudaGetDevice(&devid);
   if (devid < 0 || devid >= MAX_DEV) {
@@ -815,8 +485,11 @@ int launch_tc(const CUtensorMap maps[6], const TcParams& p_in, int bf, cudaStrea
   }
   DevState& ds = g_dev[devid];
   if (ds.num_sms == 0) {
-    cudaDeviceGetAttribute(&ds.num_sms, cudaDevAttrMultiProcessorCount, devid);
-    if (ds.num_sms <= 0) ds.num_sms = 148;
+    if (cudaDeviceGetAttribute(&ds.num_sms, cudaDevAttrMultiProcessorCount, devid) != cudaSuccess || ds.num_sms <= 0) {
+      ds.num_sms = 0;
+      di_set_error("%s: cannot query the SM count of device %d", name, devid);
+      return DI_ERR_LAUNCH;
+    }
   }
   const int g_num_sms = ds.num_sms;
   if (!ds.attr_set) {
@@ -830,11 +503,6 @@ int launch_tc(const CUtensorMap maps[6], const TcParams& p_in, int bf, cudaStrea
       return DI_ERR_LAUNCH;
     }
     ds.attr_set = true;
-  }
-  p.sched = tc::sched_slot(stream);
-  if (!p.sched) {
-    di_set_error("%s: cannot resolve the scheduler buffer", name);
-    return DI_ERR_LAUNCH;
   }
   const int tiles = p.m_tiles * p.n_tiles;
   const int sms = (g_tc_sm_limit > 0 && g_tc_sm_limit < g_num_sms) ? g_tc_sm_limit : g_num_sms;
@@ -872,15 +540,15 @@ int linear_tc_impl(const char* name, int bf, const float* A0, int lda0, int K0, 
   const int lds[3] = {lda0, lda1, lda2}, Ks[3] = {K0, K1, K2};
   int nsrc = 1 + (K1 > 0) + (K2 > 0);
   int K = K0 + K1 + K2;
-  bool ok = al16(W_hi) && al16(W_lo) && al16(C) && ldc % 4 == 0 && (K2 == 0 || K1 > 0) && (!bias || al16(bias)) &&
+  bool ok = al16(W_hi) && al16(W_lo) && al16(C) && ldc % 4 == 0 && N % 4 == 0 && (K2 == 0 || K1 > 0) && (!bias || al16(bias)) &&
             (!res || (al16(res) && ldres % 4 == 0));
   for (int s = 0; s < nsrc; ++s) ok = ok && As[s] && Ks[s] % KE == 0 && lds[s] % 4 == 0 && al16(As[s]);
   if (!ok) {
     di_set_error("%s: shape/alignment not supported by the tensor-core path", name);
     return DI_ERR_UNSUPPORTED;
   }
-  CUtensorMap maps[6];
-  bool made = make_store_map_2d(&maps[5], C, M, N, ldc);
+  CUtensorMap maps[5];
+  bool made = true;
   for (int s = 0; s < 3 && made; ++s) {
     int u = s < nsrc ? s : 0;
     made = make_map_2d(&maps[s], As[u], M, Ks[u], lds[u]);
@@ -925,10 +593,9 @@ int conv3x3_tc_impl(const char* name, int bf, int x_nchw, const float* x, const 
     di_set_error("%s: shape/alignment not supported by the tensor-core path", name);
     return DI_ERR_UNSUPPORTED;
   }
-  CUtensorMap maps[6];
+  CUtensorMap maps[5];
   long long K = 9ll * Cin;
-  bool made = make_store_map_nhwc(&maps[5], y, N, H, W, Cout) &&
-              (x_nchw ? make_map_nchw(&maps[0], x, N, H, W, Cin, KE) : make_map_nhwc(&maps[0], x, N, H, W, Cin));
+  bool made = (x_nchw ? make_map_nchw(&maps[0], x, N, H, W, Cin, KE) : make_map_nhwc(&maps[0], x, N, H, W, Cin));
   if (made) {
     if (bf) made = make_map_2d_bf16(&maps[3], w_hi, Cout, K) && make_map_2d_bf16(&maps[4], w_lo, Cout, K);
     else made = make_map_2d(&maps[3], (const float*)w_hi, Cout, K, K) && make_map_2d(&maps[4], (const float*)w_lo, Cout, K, K);
@@ -966,7 +633,7 @@ int di_tc_set_mode(int mode) {
   return DI_OK;
 }
 // Persistent tensor-core grids use at most n CTAs (0 = all SMs): with several frames in flight the other streams'
-// small kernels then always find a free SM.  The dynamic tile scheduler makes any grid size correct.
+// small kernels then always find a free SM.  The tiles are strided over the grid, so any grid size is correct.
 int di_tc_set_sm_limit(int n) {
   DI_CHECK_ARG(n >= 0, "di_tc_set_sm_limit: n must be >= 0");
   g_tc_sm_limit = n;
@@ -981,7 +648,7 @@ int di_tc_debug_read(long long* host_buf) {
   return DI_OK;
 }
 
-// Tensor-core (tcgen05 + TMA) versions of di_linear_f32: C = act([A0|A1|A2] W^T + bias + res).
+// Tensor-core (wgmma + TMA) versions of di_linear_f32: C = act([A0|A1|A2] W^T + bias + res).
 //   di_linear_tc_f32 : 3xTF32.  W_hi / W_lo fp32 [N, K]: hi = tf32(W), lo = W - hi.        every K_s % 32 == 0
 //   di_linear_tcb_f32: bf16 split.  W_hi / W_mid bf16 [N, K]: hi = bf16(W), mid = bf16(W - hi).  every K_s % 64 == 0
 // Common constraints: lda % 4 == 0, ldc % 4 == 0, 16-byte aligned pointers.  Return DI_ERR_UNSUPPORTED (-3) when a

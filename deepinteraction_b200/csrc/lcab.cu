@@ -572,12 +572,16 @@ lcab_window_bf16_kernel(const float* __restrict__ q, int ldq, const float* __res
 
 // ------------------------------------------------------------------------------------------------
 // Same kernel for PRE-SPLIT operands: q, k (kind 1) and v (kind 2) were written by the producing dense layer's
-// epilogue already as bf16 (hi, mid) words (gemm_tc.cu split_block), 4 bytes per value at the value's own position.
+// epilogue already as bf16 (hi, mid) words (gemm_tc.cu), 4 bytes per value at the value's own position.
 // The two conversion passes, one barrier per stage and the packed-V buffer disappear: stages go straight from
 // cp.async to fragments (LDS.64 for Q/K, ldmatrix.x4.trans for V).
+// PLANAR: q, k, v in the planar format (split kind 3, C = 128: per pixel 64 hi words | 64 mid words).  A 32-channel
+// stage then holds per pixel 16 hi words | 16 mid words; fragments take the hi and mid word of a channel pair from the
+// two halves, and the ldmatrix.trans rows of V are the 8-channel groups of either half.
 // ------------------------------------------------------------------------------------------------
 constexpr int VSTR2 = 36;                                            // V chunk pixel stride: 8 ldmatrix rows -> 32 distinct banks
 
+template <bool PLANAR>
 __global__ void __launch_bounds__(256, 1)
 lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
                         const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
@@ -597,11 +601,14 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
     const int c0 = (is_k ? stage : stage - nchunk) * MCH;
     float* dst = smem + (stage & 1) * BSTAGE_WORDS;
     const int pstr = is_k ? BSTR : VSTR2;
+    // source word of the stage's 16-byte piece c4: kind 1 / 2 keep a channel's position; planar: 4 pieces of hi
+    // words (c0 / 2 ..), then 4 pieces of mid words (64 + c0 / 2 ..)
+    auto src_word = [&](int c4) { return PLANAR ? (c4 < 4 ? c0 / 2 + c4 * 4 : 64 + c0 / 2 + (c4 - 4) * 4) : c0 + c4 * 4; };
     for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
       int px = i / (MCH / 4), c4 = i % (MCH / 4);
       int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
       bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
-      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
+      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + src_word(c4) : src;
       cp_async16(dst + px * pstr + c4 * 4, gp, ok);
     }
     if (is_k) {
@@ -610,11 +617,15 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
         int px = i / (MCH / 4), c4 = i % (MCH / 4);
         int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
         bool ok = gy < H && gx < W;
-        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
+        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + src_word(c4) : q;
         cp_async16(qd + px * BSTR + c4 * 4, gp, ok);
       }
     }
     cp_async_commit();
+  };
+  // (hi, mid) words of channel pair j of a pixel row in a K / Q stage
+  auto pair_at = [](const uint32_t* row, int j) -> uint2 {
+    return PLANAR ? make_uint2(row[j], row[16 + j]) : *reinterpret_cast<const uint2*>(row + 2 * j);
   };
 
   const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
@@ -641,10 +652,10 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
       for (int ks = 0; ks < MCH / 16; ++ks) {
         uint32_t ah[4], am[4];
         {
-          const uint2 a0 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t) * 2);
-          const uint2 a1 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t) * 2);
-          const uint2 a2 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t + 4) * 2);
-          const uint2 a3 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t + 4) * 2);
+          const uint2 a0 = pair_at(qw + g * BSTR, ks * 8 + t);
+          const uint2 a1 = pair_at(qw + (MQ_COLS + g) * BSTR, ks * 8 + t);
+          const uint2 a2 = pair_at(qw + g * BSTR, ks * 8 + t + 4);
+          const uint2 a3 = pair_at(qw + (MQ_COLS + g) * BSTR, ks * 8 + t + 4);
           ah[0] = a0.x; am[0] = a0.y; ah[1] = a1.x; am[1] = a1.y;
           ah[2] = a2.x; am[2] = a2.y; ah[3] = a3.x; am[3] = a3.y;
         }
@@ -655,9 +666,9 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
           uint2 b0[4], b1[4];
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
-            const uint32_t* kp = kw + ((wy + 2 * r2 + (u >> 1)) * MT_COLS + wx + (u & 1) * 8 + g) * BSTR + (ks * 8 + t) * 2;
-            b0[u] = *reinterpret_cast<const uint2*>(kp);
-            b1[u] = *reinterpret_cast<const uint2*>(kp + 8);
+            const uint32_t* kp = kw + ((wy + 2 * r2 + (u >> 1)) * MT_COLS + wx + (u & 1) * 8 + g) * BSTR;
+            b0[u] = pair_at(kp, ks * 8 + t);
+            b1[u] = pair_at(kp, ks * 8 + t + 4);
           }
 #pragma unroll
           for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
@@ -715,13 +726,15 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
       }
     } else {
       // ---------------- O[chunk] = P V[chunk] ----------------
-      // V arrives pre-split in 8-channel groups [4 hi words | 4 mid words]; ldmatrix.trans turns the [key][channel]
-      // rows into the (k = key pair, n = channel) B fragments: matrices 0/1 = keys 0-7 / 8-15 hi, 2/3 = the mid parts.
+      // V arrives pre-split in 8-channel groups [4 hi words | 4 mid words] (planar: hi groups in words 0..15, mid groups
+      // in 16..31); ldmatrix.trans turns the [key][channel] rows into the (k = key pair, n = channel) B fragments:
+      // matrices 0/1 = keys 0-7 / 8-15 hi, 2/3 = the mid parts.
+      constexpr int MID_OFF = PLANAR ? 16 : 4, NB_STEP = PLANAR ? 4 : 8;
       float O[MCH / 8][4];
 #pragma unroll
       for (int nb = 0; nb < MCH / 8; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
       const uint32_t vbase = (uint32_t)__cvta_generic_to_shared(buf) +
-                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * 4) * 4);
+                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * MID_OFF) * 4);
 #pragma unroll
       for (int r = 0; r < 10; ++r) {
         uint32_t bh0[MCH / 8], bh1[MCH / 8], bm0[MCH / 8], bm1[MCH / 8];
@@ -729,7 +742,7 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
         for (int nb = 0; nb < MCH / 8; ++nb)
           asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
                        : "=r"(bh0[nb]), "=r"(bh1[nb]), "=r"(bm0[nb]), "=r"(bm1[nb])
-                       : "r"(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * 8) * 4)));
+                       : "r"(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * NB_STEP) * 4)));
 #pragma unroll
         for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Pm[r], bh0[nb], bh1[nb]);
 #pragma unroll
@@ -843,12 +856,40 @@ int di_lcab_window_pre_f32(const float* q, int ldq, const float* k, int ldk, con
   dim3 mgrid(di_cdiv(W, MQ_COLS), di_cdiv(H, MQ_ROWS), N);
   size_t smem = 2ull * BSTAGE_WORDS * sizeof(float);
   static DiSmemOnce once{};
-  if (!di_smem_once(once, lcab_window_pre_kernel, (int)smem)) {
+  if (!di_smem_once(once, lcab_window_pre_kernel<false>, (int)smem)) {
     di_set_error("di_lcab_window_pre_f32: cannot reserve shared memory");
     return DI_ERR_LAUNCH;
   }
-  lcab_window_pre_kernel<<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, 1.0f / sqrtf((float)C));
+  lcab_window_pre_kernel<false><<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, 1.0f / sqrtf((float)C));
   DI_CHECK_LAUNCH("di_lcab_window_pre_f32");
+  return DI_OK;
+}
+
+// 9x9 window attention for PLANAR pre-split operands (di_linear_tcb_split_f32 split_kind 3): q, k, v point at [N*H*W]
+// pixels with a per-pixel stride of ld* 32-bit words, each pixel holding 128 bf16 hi values followed by 128 bf16 mid
+// values (x = hi + mid to 16 mantissa bits).  out: fp32 [N, H, W, ldo], C = 128 channels written.
+int di_lcab_window_tc_f32(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, float* out, int ldo,
+                          int N, int H, int W, int C, cudaStream_t stream) {
+  DI_CHECK_ARG(q && k && v && out && N > 0 && H > 0 && W > 0, "di_lcab_window_tc_f32: bad argument");
+  if (C != 128) {
+    di_set_error("di_lcab_window_tc_f32: C must be 128 (got %d)", C);
+    return DI_ERR_UNSUPPORTED;
+  }
+  DI_CHECK_ARG(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldo % 4 == 0 && ldq >= 128 && ldk >= 128 && ldv >= 128 && ldo >= 128,
+               "di_lcab_window_tc_f32: strides must be multiples of 4 words and >= 128");
+  DI_CHECK_ARG(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) % 16 == 0,
+               "di_lcab_window_tc_f32: pointers must be 16-byte aligned");
+  dim3 mgrid(di_cdiv(W, MQ_COLS), di_cdiv(H, MQ_ROWS), N);
+  size_t smem = 2ull * BSTAGE_WORDS * sizeof(float);
+  static DiSmemOnce once{};
+  if (!di_smem_once(once, lcab_window_pre_kernel<true>, (int)smem)) {
+    di_set_error("di_lcab_window_tc_f32: cannot reserve shared memory");
+    return DI_ERR_LAUNCH;
+  }
+  lcab_window_pre_kernel<true><<<mgrid, 256, smem, stream>>>(static_cast<const float*>(q), ldq, static_cast<const float*>(k), ldk,
+                                                             static_cast<const float*>(v), ldv, out, ldo, H, W, C,
+                                                             1.0f / sqrtf((float)C));
+  DI_CHECK_LAUNCH("di_lcab_window_tc_f32");
   return DI_OK;
 }
 

@@ -1,392 +1,18 @@
-// The five 1x1 Conv(+folded BN)+ReLU projections of LocalContextAttentionBlock as ONE tcgen05 launch
+// The five 1x1 Conv(+folded BN)+ReLU projections of LocalContextAttentionBlock
 // (reference projects/mmdet3d_plugin/models/utils/encoder_utils.py:92-131: query_project = 2 layers on the target map,
 // key_project = 2 layers and value_project = 1 layer on the source map):
 //
 //     q = relu(W_q2 relu(W_q1 x_t + b_q1) + b_q2)      k = relu(W_k2 relu(W_k1 x_s + b_k1) + b_k2)      v = relu(W_v x_s + b_v)
 //
-// written directly in the planar bf16 hi|mid operand format of the tcgen05 window kernel (lcab_tc.cu).  The first-stage
-// activations q1 / k1 never leave the SM: a persistent CTA owns one ROLE (q chain, k chain or v; CTAs dealt 2 : 2 : 1) and keeps
-// that role's weights resident in shared memory (W1 slice + W2 slice, bf16 hi + mid, 128 KB); per 128-row tile
-//   x tile (TMA, fp32) -> splitter warps: bf16 hi/mid -> TENSOR MEMORY -> GEMM 1 (tcgen05.mma, A from TMEM)
-//   -> epilogue warps: bias + ReLU + hi/mid split, written back to tensor memory as the A operand of
-//   GEMM 2 (same accumulator columns) -> epilogue: bias + ReLU + planar split -> swizzled staging -> TMA store.
-// HBM traffic of the module's projections: x read once per role (twice out of L2) + q, k, v written once = 4 F instead
-// of the 8 F of the unfused chain (q1 | k1 | v GEMM, then q and k GEMMs).  Same split-product arithmetic as gemm_tc.cu
-// (A_mid W_hi + A_hi W_mid + A_hi W_hi on kind::f16, fp32 accumulate), so results equal the unfused path bit for bit.
-//
-// Warp roles as in gemm_tc.cu: warp 0 TMA producer + dynamic tile scheduler (one counter per role), warp 1 MMA issuer,
-// warps 2-5 splitter, warps 6-9 epilogue.  The MMA issuer is software-pipelined by one tile: GEMM 1 of tile t+1 is
-// issued before GEMM 2 of tile t, so the tensor pipe works while the epilogue warps turn q1 into an operand.
-//   TMEM columns: acc0 [0,128) | acc1 [128,256) | streamed-A buffers 2 x 64 [256,384) | stage-2 operand A2 [384,512)
-#include "tc_common.cuh"
-
-namespace {
-using namespace tc;
-
-constexpr int TM = 128;
-constexpr int BOX = 16384;                         // one 128-row x 128-byte operand box
-constexpr int AL = 2 * BOX;                        // fp32 landing buffer of one 64-wide K chunk (two 32-column boxes)
-constexpr int S = 2;                               // landing stages == TMEM A buffers
-constexpr int W1_OFF = 0, W2_OFF = 4 * BOX, RING_OFF = 8 * BOX, EP_OFF = RING_OFF + S * AL;
-constexpr int EP_BYTES = 4 * 2 * 4096;
-constexpr int BAR_OFF = EP_OFF + EP_BYTES, BIAS_OFF = BAR_OFF + 256, TQ_OFF = BIAS_OFF + 1024;
-constexpr int PJ_SMEM_BYTES = TQ_OFF + 64;
-static_assert(PJ_SMEM_BYTES <= 232448, "projection kernel exceeds the 227 KB shared-memory limit");
-constexpr int TQD = 4;
-constexpr int PJ_THREADS = 320;
-constexpr uint32_t IDESC_BF16 = (1u << 4) | (1u << 7) | (1u << 10) | ((128u >> 3) << 17) | ((128u >> 4) << 24);
-constexpr uint32_t A_COL = 256, A2_COL = 384;
-
-struct PjParams {
-  int M, m_tiles;
-  int src[3];                 // A source (0 = target map, 1 = source map) of role q / k / v
-  const float* bias1;         // [384]
-  const float* bias2;         // [256]
-  int* sched;                 // 16 ints: [role] tile counters, [15] done counter
-  int n_chain;                // CTAs per chain role (q, k); the rest of the grid serves v
-};
-
-__global__ void __launch_bounds__(PJ_THREADS, 1)
-lcab_proj_kernel(const __grid_constant__ CUtensorMap mapX0, const __grid_constant__ CUtensorMap mapX1,
-                 const __grid_constant__ CUtensorMap mapW1h, const __grid_constant__ CUtensorMap mapW1m,
-                 const __grid_constant__ CUtensorMap mapW2h, const __grid_constant__ CUtensorMap mapW2m,
-                 const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                 const __grid_constant__ CUtensorMap mapV, const PjParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base = smem_u32(smem_raw);
-  uint8_t* base_ptr = smem_raw;
-  if ((base & 1023u) != 0u) __trap();
-  const uint32_t bars = base + BAR_OFF;
-  auto full = [&](int s) { return bars + 8u * s; };               // landing stage s filled (TMA)
-  auto empty = [&](int s) { return bars + 16u + 8u * s; };        // landing stage s read by the 4 splitter warps
-  auto a_ready = [&](int b) { return bars + 32u + 8u * b; };      // TMEM A buffer b written (4 splitter warps)
-  auto a_free = [&](int b) { return bars + 48u + 8u * b; };       // MMAs that read A buffer b retired (commit)
-  auto acc_full = [&](int a) { return bars + 64u + 8u * a; };     // GEMM 1 of the tile in accumulator a done
-  auto acc2_full = [&](int a) { return bars + 80u + 8u * a; };    // GEMM 2 done
-  auto acc_empty = [&](int a) { return bars + 96u + 8u * a; };    // final epilogue has drained accumulator a
-  const uint32_t a2_ready = bars + 112, a2_free = bars + 120, w_full = bars + 128, tmem_slot = bars + 136;
-  auto tq_full = [&](int i) { return bars + 144u + 8u * i; };
-  auto tq_empty = [&](int i) { return bars + 176u + 8u * i; };
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(base_ptr + BAR_OFF + 136);
-  volatile int* tq = reinterpret_cast<volatile int*>(base_ptr + TQ_OFF);
-  float* bias_s = reinterpret_cast<float*>(base_ptr + BIAS_OFF);   // [0,128) stage-1 bias slice, [128,256) stage-2
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  // CTAs are dealt 2 : 2 : 1 to the roles: a chain role (two GEMMs + two epilogues per tile) costs twice the v role
-  const int role = (int)blockIdx.x < p.n_chain ? 0 : ((int)blockIdx.x < 2 * p.n_chain ? 1 : 2);
-  const bool chain = role < 2;
-  if (threadIdx.x == 0) {
-    for (int s = 0; s < S; ++s) {
-      mbar_init(full(s), 1);
-      mbar_init(empty(s), 4);
-      mbar_init(a_ready(s), 4);
-      mbar_init(a_free(s), 1);
-      mbar_init(acc_full(s), 1);
-      mbar_init(acc2_full(s), 1);
-      mbar_init(acc_empty(s), 4);
-    }
-    mbar_init(a2_ready, 4);
-    mbar_init(a2_free, 1);
-    mbar_init(w_full, 1);
-    for (int i = 0; i < TQD; ++i) {
-      mbar_init(tq_full(i), 1);
-      mbar_init(tq_empty(i), 9);                    // MMA warp + 4 splitter warps + 4 epilogue warps
-    }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (threadIdx.x < 256) bias_s[threadIdx.x] = threadIdx.x < 128 ? __ldg(p.bias1 + role * 128 + threadIdx.x)
-                                                                   : (chain ? __ldg(p.bias2 + role * 128 + threadIdx.x - 128) : 0.f);
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
-
-  auto take_tile = [&](int tl) -> int {
-    const int i = tl % TQD;
-    mbar_wait(tq_full(i), (tl / TQD) & 1);
-    const int tile = tq[i];
-    __syncwarp();
-    if (lane == 0) mbar_arrive(tq_empty(i));
-    return tile;
-  };
-
-  if (warp == 0) {
-    // ---------------- tile scheduler + TMA producer ----------------
-    if (lane == 0) {
-      const CUtensorMap* mx = p.src[role] == 0 ? &mapX0 : &mapX1;
-      int it = 0, published = 0;
-      bool exhausted = false;
-      auto publish = [&]() {
-        const int i = published % TQD;
-        if (published >= TQD) mbar_wait(tq_empty(i), ((published / TQD) - 1) & 1);
-        int tile = atomicAdd(p.sched + role, 1);
-        if (tile >= p.m_tiles) tile = -1;
-        if (tile >= 0)                                  // L2 prefetch of the tile's rows
-          for (int c = 0; c < 4; ++c) tma_prefetch_2d(mx, c * 32, tile * TM);
-        tq[i] = tile;
-        mbar_arrive(tq_full(i));
-        exhausted = tile < 0;
-        ++published;
-      };
-      publish();
-      for (int n = 0;; ++n) {
-        const int tile = tq[n % TQD];
-        if (tile < 0) break;
-        for (int kc = 0; kc < 2; ++kc, ++it) {
-          const int s = it % S;
-          if (it >= S) mbar_wait(empty(s), ((it / S) - 1) & 1);
-          const uint32_t st = base + RING_OFF + s * AL;
-          mbar_expect_tx(full(s), AL);
-          tma_load_2d(st, mx, full(s), kc * 64, tile * TM);
-          tma_load_2d(st + BOX, mx, full(s), kc * 64 + 32, tile * TM);
-        }
-        if (n == 0) {                                   // resident weights, after the first tile's A chunks
-          mbar_expect_tx(w_full, (chain ? 8 : 4) * BOX);
-          for (int kc = 0; kc < 2; ++kc) {
-            tma_load_2d(base + W1_OFF + kc * BOX, &mapW1h, w_full, kc * 64, role * 128);
-            tma_load_2d(base + W1_OFF + (2 + kc) * BOX, &mapW1m, w_full, kc * 64, role * 128);
-            if (chain) {
-              tma_load_2d(base + W2_OFF + kc * BOX, &mapW2h, w_full, kc * 64, role * 128);
-              tma_load_2d(base + W2_OFF + (2 + kc) * BOX, &mapW2m, w_full, kc * 64, role * 128);
-            }
-          }
-        }
-        while (!exhausted && published <= n + 2) publish();
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer (software-pipelined by one tile) ----------------
-    int it = 0;
-    bool pending = false;                               // GEMM 2 of the previous tile still to be issued
-    for (int tl = 0;; ++tl) {
-      const int tile = take_tile(tl);
-      if (tile >= 0) {
-        if (tl == 0) mbar_wait(w_full, 0);
-        const int a = tl & 1;
-        if (tl >= 2) mbar_wait(acc_empty(a), ((tl >> 1) - 1) & 1);
-        const uint32_t acc = tmem_base + (uint32_t)(a * 128);
-        for (int kc = 0; kc < 2; ++kc, ++it) {
-          const int b = it % S;
-          mbar_wait(a_ready(b), (it / S) & 1);
-          tc_fence_after();
-          if (elect_one()) {
-            const uint32_t ta = tmem_base + A_COL + (uint32_t)(b * 64);
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t w_hi = umma_desc(base + W1_OFF + kc * BOX + k * 32), w_mid = umma_desc(base + W1_OFF + (2 + kc) * BOX + k * 32);
-              umma_bf16_ts(acc, ta + 32u + (uint32_t)(k * 8), w_hi, IDESC_BF16, (kc | k) != 0);   // A_mid * W_hi
-              umma_bf16_ts(acc, ta + (uint32_t)(k * 8), w_mid, IDESC_BF16, 1);                    // A_hi * W_mid
-              umma_bf16_ts(acc, ta + (uint32_t)(k * 8), w_hi, IDESC_BF16, 1);                     // A_hi * W_hi
-            }
-            umma_commit(a_free(b));
-            if (kc == 1) umma_commit(acc_full(a));
-          }
-          __syncwarp();
-        }
-      }
-      if (pending) {                                    // GEMM 2 of tile tl - 1: A = relu(stage 1) from tensor memory
-        const int a = (tl - 1) & 1;
-        mbar_wait(a2_ready, (tl - 1) & 1);
-        tc_fence_after();
-        if (elect_one()) {
-          const uint32_t acc = tmem_base + (uint32_t)(a * 128);
-#pragma unroll
-          for (int kc = 0; kc < 2; ++kc)
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint32_t ta = tmem_base + A2_COL + (uint32_t)(kc * 64 + k * 8);
-              const uint64_t w_hi = umma_desc(base + W2_OFF + kc * BOX + k * 32), w_mid = umma_desc(base + W2_OFF + (2 + kc) * BOX + k * 32);
-              umma_bf16_ts(acc, ta + 32u, w_hi, IDESC_BF16, (kc | k) != 0);
-              umma_bf16_ts(acc, ta, w_mid, IDESC_BF16, 1);
-              umma_bf16_ts(acc, ta, w_hi, IDESC_BF16, 1);
-            }
-          umma_commit(a2_free);
-          umma_commit(acc2_full(a));
-        }
-        __syncwarp();
-      }
-      pending = tile >= 0 && chain;
-      if (tile < 0) break;
-    }
-  } else if (warp < 6) {
-    // ---------------- splitter (warps 2..5): fp32 landing chunk -> bf16 hi / mid -> tensor memory ----------------
-    const int qd = warp & 3;
-    const int row = qd * 32 + lane;
-    int it = 0;
-    for (int tl = 0;; ++tl) {
-      if (take_tile(tl) < 0) break;
-      for (int kc = 0; kc < 2; ++kc, ++it) {
-        const int s = it % S;
-        uint32_t hi[32], lo[32];
-        mbar_wait(full(s), (it / S) & 1);
-        const uint8_t* arow = base_ptr + RING_OFF + s * AL + row * 128;
-#pragma unroll
-        for (int h = 0; h < 2; ++h)
-#pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 x = *reinterpret_cast<const float4*>(arow + h * BOX + ((j ^ (row & 7)) << 4));
-            const uint32_t h01 = pack_bf16x2(x.x, x.y), h23 = pack_bf16x2(x.z, x.w);
-            hi[h * 16 + 2 * j] = h01;
-            hi[h * 16 + 2 * j + 1] = h23;
-            lo[h * 16 + 2 * j] = pack_bf16x2(x.x - __uint_as_float(h01 << 16), x.y - __uint_as_float(h01 & 0xFFFF0000u));
-            lo[h * 16 + 2 * j + 1] = pack_bf16x2(x.z - __uint_as_float(h23 << 16), x.w - __uint_as_float(h23 & 0xFFFF0000u));
-          }
-        __syncwarp();
-        if (lane == 0) mbar_arrive(empty(s));            // landing buffer read
-        if (it >= S) mbar_wait(a_free(s), ((it / S) - 1) & 1);
-        tc_fence_after();
-        const uint32_t ta = tmem_base + ((uint32_t)(qd * 32) << 16) + A_COL + (uint32_t)(s * 64);
-        tmem_st32(ta, hi);
-        tmem_st32(ta + 32u, lo);
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_ready(s));
-      }
-    }
-  } else {
-    // ---------------- epilogue (warps 6..9) ----------------
-    const int q = warp & 3;
-    const uint32_t my_ep = base + EP_OFF + (uint32_t)((warp - 6) * 2) * 4096u;
-    const uint32_t tl_base = tmem_base + ((uint32_t)(q * 32) << 16);
-    const CUtensorMap* mo = role == 0 ? &mapQ : (role == 1 ? &mapK : &mapV);
-    int chunk = 0;
-    for (int tl = 0;; ++tl) {
-      const int tile = take_tile(tl);
-      if (tile < 0) break;
-      const int a = tl & 1;
-      const uint32_t tacc = tl_base + (uint32_t)(a * 128);
-      mbar_wait(acc_full(a), (tl >> 1) & 1);
-      tc_fence_after();
-      if (chain) {
-        // stage-1 epilogue: relu(acc + b1) -> bf16 hi / mid -> A2 (chunk c = 64 k-values: 32 hi columns | 32 mid columns)
-        if (tl >= 1) mbar_wait(a2_free, (tl - 1) & 1);   // GEMM 2 of the previous tile has read A2
-        tc_fence_after();
-#pragma unroll 1
-        for (int j = 0; j < 4; ++j) {
-          float v[32];
-          tmem_ld32_nowait(tacc + (uint32_t)(j * 32), v);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-          uint32_t w[32];
-#pragma unroll
-          for (int i = 0; i < 16; ++i) {
-            const float x0 = fmaxf(v[2 * i] + bias_s[j * 32 + 2 * i], 0.f), x1 = fmaxf(v[2 * i + 1] + bias_s[j * 32 + 2 * i + 1], 0.f);
-            const uint32_t h = pack_bf16x2(x0, x1);
-            w[i] = h;
-            w[16 + i] = pack_bf16x2(x0 - __uint_as_float(h << 16), x1 - __uint_as_float(h & 0xFFFF0000u));
-          }
-          const uint32_t ta = tl_base + A2_COL + (uint32_t)((j >> 1) * 64 + (j & 1) * 16);
-          asm volatile(
-              "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(ta),
-              "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3]), "r"(w[4]), "r"(w[5]), "r"(w[6]), "r"(w[7]), "r"(w[8]), "r"(w[9]),
-              "r"(w[10]), "r"(w[11]), "r"(w[12]), "r"(w[13]), "r"(w[14]), "r"(w[15])
-              : "memory");
-          asm volatile(
-              "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(ta + 32u),
-              "r"(w[16]), "r"(w[17]), "r"(w[18]), "r"(w[19]), "r"(w[20]), "r"(w[21]), "r"(w[22]), "r"(w[23]), "r"(w[24]),
-              "r"(w[25]), "r"(w[26]), "r"(w[27]), "r"(w[28]), "r"(w[29]), "r"(w[30]), "r"(w[31])
-              : "memory");
-        }
-        asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a2_ready);
-        mbar_wait(acc2_full(a), (tl >> 1) & 1);
-        tc_fence_after();
-      }
-      // final epilogue: relu(acc + b) -> planar bf16 hi | mid words -> swizzled staging -> TMA store
-      const float* bs = bias_s + (chain ? 128 : 0);
-#pragma unroll 1
-      for (int h = 0; h < 2; ++h) {
-        float v0[32], v1[32];
-        tmem_ld32_nowait(tacc + (uint32_t)(h * 64), v0);
-        tmem_ld32_nowait(tacc + (uint32_t)(h * 64 + 32), v1);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        if (h == 1) {                                     // last TMEM read of this tile: release the accumulator
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(acc_empty(a));
-        }
-        uint32_t hw[32], mw[32];
-#pragma unroll
-        for (int i = 0; i < 16; ++i) {
-          const float x0 = fmaxf(v0[2 * i] + bs[h * 64 + 2 * i], 0.f), x1 = fmaxf(v0[2 * i + 1] + bs[h * 64 + 2 * i + 1], 0.f);
-          const float y0 = fmaxf(v1[2 * i] + bs[h * 64 + 32 + 2 * i], 0.f), y1 = fmaxf(v1[2 * i + 1] + bs[h * 64 + 32 + 2 * i + 1], 0.f);
-          hw[i] = pack_bf16x2(x0, x1);
-          mw[i] = pack_bf16x2(x0 - __uint_as_float(hw[i] << 16), x1 - __uint_as_float(hw[i] & 0xFFFF0000u));
-          hw[16 + i] = pack_bf16x2(y0, y1);
-          mw[16 + i] = pack_bf16x2(y0 - __uint_as_float(hw[16 + i] << 16), y1 - __uint_as_float(hw[16 + i] & 0xFFFF0000u));
-        }
-#pragma unroll
-        for (int part = 0; part < 2; ++part) {
-          const uint32_t* src = part == 0 ? hw : mw;
-          const uint32_t buf = my_ep + (uint32_t)(chunk & 1) * 4096u;
-          if (lane == 0) asm volatile("cp.async.bulk.wait_group.read 1;" ::: "memory");
-          __syncwarp();
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            asm volatile("st.shared.v4.b32 [%0], {%1, %2, %3, %4};" ::"r"(buf + lane * 128 + ((j ^ (lane & 7)) << 4)),
-                         "r"(src[4 * j]), "r"(src[4 * j + 1]), "r"(src[4 * j + 2]), "r"(src[4 * j + 3])
-                         : "memory");
-          asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          __syncwarp();
-          if (lane == 0) {
-            tma_store_2d(mo, buf, part * 64 + h * 32, tile * TM + 32 * q);     // hi words [0,64), mid words [64,128)
-            asm volatile("cp.async.bulk.commit_group;" ::: "memory");
-          }
-          ++chunk;
-        }
-      }
-    }
-    if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    __threadfence();
-    if (atomicAdd(p.sched + 15, 1) == (int)gridDim.x - 1) {
-      for (int i = 0; i < 16; ++i) p.sched[i] = 0;
-      __threadfence();
-    }
-  }
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
-  }
-}
-
-bool map_2d(CUtensorMap* m, CUtensorMapDataType dt, int esz, const void* ptr, long long rows, long long cols, long long ld,
-            int box_c, int box_r, CUtensorMapL2promotion prom) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld * esz};
-  cuuint32_t box[2] = {(cuuint32_t)box_c, (cuuint32_t)box_r};
-  cuuint32_t estr[2] = {1, 1};
-  return enc(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-             CU_TENSOR_MAP_SWIZZLE_128B, prom, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
-struct PjDev {
-  int num_sms = 0;
-  bool attr_set = false;
-};
-PjDev g_pj_dev[64];
-int g_pj_sm_limit = 0;
-
-}  // namespace
+// written directly in the planar bf16 hi|mid operand format of the window kernel (di_lcab_window_tc_f32), as a chain of
+// five launches of the bf16-split tensor-core GEMM (gemm_tc.cu).  Each layer is the same launch the unfused chain makes,
+// so results equal the unfused path bit for bit.  The first-stage activations q1 / k1 are written into the q / k output
+// buffers and the second stage runs IN PLACE over them: with N = 128 there is one column tile, and a CTA has read all
+// A rows of a tile (every K chunk) before its epilogue writes that tile's rows, while no other CTA touches those rows.
+#include "common.cuh"
+#include "di_b200.h"
 
 extern "C" {
-
-int di_lcab_proj_set_sm_limit(int n) {
-  DI_CHECK_ARG(n >= 0, "di_lcab_proj_set_sm_limit: n must be >= 0");
-  g_pj_sm_limit = n;
-  return DI_OK;
-}
 
 // x_t / x_s [M, 128] fp32 rows (leading dimensions ld_t / ld_s; x_s == x_t for self attention).
 // W1_hi / W1_mid [384, 128] bf16 = rows (q1 | k1 | v), b1 [384]; W2_hi / W2_mid [256, 128] = rows (q2 | k2), b2 [256]
@@ -399,63 +25,29 @@ int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, con
   DI_CHECK_ARG(ld_t % 4 == 0 && ld_s % 4 == 0 && ld_t >= 128 && ld_s >= 128, "di_lcab_proj_f32: leading dimensions");
   DI_CHECK_ARG((((uintptr_t)x_t | (uintptr_t)x_s | (uintptr_t)W1_hi | (uintptr_t)W1_mid | (uintptr_t)W2_hi | (uintptr_t)W2_mid |
                  (uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "di_lcab_proj_f32: pointers must be 16-byte aligned");
-  int devid = 0;
-  cudaGetDevice(&devid);
-  if (devid < 0 || devid >= 64) {
-    di_set_error("di_lcab_proj_f32: device ordinal %d not supported", devid);
-    return DI_ERR_UNSUPPORTED;
+  DI_CHECK_ARG(q != k && q != v && k != v, "di_lcab_proj_f32: q, k, v must be distinct buffers");
+  constexpr size_t WB = 128 * 128 * 2;               // bytes of one 128 x 128 bf16 weight block
+  auto w = [&](const void* p, int blk) { return static_cast<const void*>(static_cast<const char*>(p) + blk * WB); };
+  struct Layer {
+    const float* a; int lda; const void* wh; const void* wm; const float* b; float* out; int kind;
+  };
+  const Layer chain[5] = {
+      {x_t, ld_t, w(W1_hi, 0), w(W1_mid, 0), b1, q, 0},            // q1 = relu(W_q1 x_t + b_q1)  -> q (fp32)
+      {q, 128, w(W2_hi, 0), w(W2_mid, 0), b2, q, 3},               // q  = relu(W_q2 q1 + b_q2)   -> q (planar, in place)
+      {x_s, ld_s, w(W1_hi, 1), w(W1_mid, 1), b1 + 128, k, 0},      // k1 = relu(W_k1 x_s + b_k1)  -> k (fp32)
+      {k, 128, w(W2_hi, 1), w(W2_mid, 1), b2 + 128, k, 3},         // k  = relu(W_k2 k1 + b_k2)   -> k (planar, in place)
+      {x_s, ld_s, w(W1_hi, 2), w(W1_mid, 2), b1 + 256, v, 3},      // v  = relu(W_v x_s + b_v)    -> v (planar)
+  };
+  for (const Layer& l : chain) {
+    const int rc = di_linear_tcb_split_f32(l.a, l.lda, 128, nullptr, 0, 0, nullptr, 0, 0, l.wh, l.wm, l.b, nullptr, 0, 0,
+                                           l.out, 128, M, 128, DI_ACT_RELU, 0, l.kind, stream);
+    if (rc != DI_OK) return rc;
   }
-  PjDev& ds = g_pj_dev[devid];
-  if (ds.num_sms == 0) {
-    cudaDeviceGetAttribute(&ds.num_sms, cudaDevAttrMultiProcessorCount, devid);
-    if (ds.num_sms <= 0) ds.num_sms = 148;
-  }
-  if (!ds.attr_set) {
-    if (cudaFuncSetAttribute(lcab_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM_BYTES) != cudaSuccess) {
-      di_set_error("di_lcab_proj_f32: cannot reserve %d bytes of shared memory", PJ_SMEM_BYTES);
-      return DI_ERR_LAUNCH;
-    }
-    ds.attr_set = true;
-  }
-  CUtensorMap mx0, mx1, w1h, w1m, w2h, w2m, mq, mk, mv;
-  const auto F32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
-  const auto BF = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16;
-  const auto P128 = CU_TENSOR_MAP_L2_PROMOTION_L2_128B;
-  const auto PN = CU_TENSOR_MAP_L2_PROMOTION_NONE;
-  bool ok = map_2d(&mx0, F32, 4, x_t, M, 128, ld_t, 32, 128, P128) && map_2d(&mx1, F32, 4, x_s, M, 128, ld_s, 32, 128, P128) &&
-            map_2d(&w1h, BF, 2, W1_hi, 384, 128, 128, 64, 128, P128) && map_2d(&w1m, BF, 2, W1_mid, 384, 128, 128, 64, 128, P128) &&
-            map_2d(&w2h, BF, 2, W2_hi, 256, 128, 128, 64, 128, P128) && map_2d(&w2m, BF, 2, W2_mid, 256, 128, 128, 64, 128, P128) &&
-            map_2d(&mq, F32, 4, q, M, 128, 128, 32, 32, PN) && map_2d(&mk, F32, 4, k, M, 128, 128, 32, 32, PN) &&
-            map_2d(&mv, F32, 4, v, M, 128, 128, 32, 32, PN);
-  if (!ok) {
-    di_set_error("di_lcab_proj_f32: cuTensorMapEncodeTiled failed");
-    return DI_ERR_LAUNCH;
-  }
-  PjParams p{};
-  p.M = M;
-  p.m_tiles = di_cdiv(M, TM);
-  p.src[0] = 0;
-  p.src[1] = 1;
-  p.src[2] = 1;
-  p.bias1 = b1;
-  p.bias2 = b2;
-  p.sched = tc::sched_slot(stream);
-  if (!p.sched) {
-    di_set_error("di_lcab_proj_f32: cannot resolve the scheduler buffer");
-    return DI_ERR_LAUNCH;
-  }
-  const int sms = (g_pj_sm_limit > 0 && g_pj_sm_limit < ds.num_sms) ? g_pj_sm_limit : ds.num_sms;
-  int grid = sms < 5 ? 5 : sms;
-  if (grid > 3 * p.m_tiles) grid = 3 * p.m_tiles < 5 ? 5 : 3 * p.m_tiles;
-  p.n_chain = (2 * grid) / 5;
-  if (p.n_chain < 1) p.n_chain = 1;
-  lcab_proj_kernel<<<grid, PJ_THREADS, PJ_SMEM_BYTES, stream>>>(mx0, mx1, w1h, w1m, w2h, w2m, mq, mk, mv, p);
-  DI_CHECK_LAUNCH("di_lcab_proj_f32");
   return DI_OK;
 }
 
 // LocalContextAttentionBlock.forward (models/utils/encoder_utils.py:119-135) for C = 128 as ONE call: the projection chain
-// (di_lcab_proj_f32) followed by the tcgen05 window kernel (di_lcab_window_tc_f32) on `stream`.  x_t / x_s [N*H*W, 128]
+// (di_lcab_proj_f32) followed by the window kernel (di_lcab_window_tc_f32) on `stream`.  x_t / x_s [N*H*W, 128]
 // fp32 pixel-major rows (x_s == x_t: self attention), folded weights as for di_lcab_proj_f32, qkv: workspace of
 // 3 * N*H*W * 128 32-bit words (16-byte aligned), out [N*H*W, ldo] fp32.  This is the entry SURVEY.md 8(b) calls
 // `di_lcab_forward`: module-boundary traffic = x_t (+ x_s) read once, out written once; q / k / v pass through `qkv` (L2).

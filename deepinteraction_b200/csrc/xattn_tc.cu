@@ -1,25 +1,20 @@
-// Query x BEV cross attention of the MMPI decoder on the Blackwell tensor cores (tcgen05 + TMEM + TMA).
+// Query x BEV cross attention of the MMPI decoder on the tensor cores (mma.sync bf16, cp.async-staged operands).
 //
 // Reference: TransformerDecoderLayer / multi_head_attention_forward, models/utils/decoder_utils.py:101-103, 466-493:
 // P = 200 object queries x HW = 32 400 BEV keys, 8 heads of 16 channels, softmax over all keys.  The K / V projection
 // (with the folded key positional term) stays a 3xTF32 GEMM; di_attn_planes_f32 then writes the operands as bf16 PLANES:
 // K and the pre-scaled queries as hi | mid | lo (x = hi + mid + lo to 24 mantissa bits: the logits go through exp, and a
-// two-plane product -- 3 * 2^-18 relative -- moved the decoder outputs by up to 3e-3), V as hi | mid.  A TMA box
-// {64 channels, rows} of a plane is a 128B-swizzled tcgen05 operand tile whose 32-byte k-slices are the heads.
+// two-plane product -- 3 * 2^-18 relative -- moved the decoder outputs by up to 3e-3), V as hi | mid.  The 16 channels
+// of a head are one k16 step of the MMA.
 //
-// CTA = (batch, query tile of 128, channel box of 64 = 4 heads, key split).  Per key tile of 64 keys:
-//   S_h[128 q x 64 keys] = Q_h K_h^T    h = 0..3: one k-step (16 channels) per head, SS-mode tcgen05.mma kind::f16,
-//                                       six-term split product (lo hi, hi lo, mid mid, mid hi, hi mid, hi hi: error
-//                                       ~2^-26) -> TMEM columns [64 h, 64 h + 64)
-//   P_h = exp(S_h - m)                  8 softmax warps (two per TMEM lane quarter, two heads each), thread = query:
-//                                       running maximum m and sum l per head in registers (online softmax), P written
-//                                       IN PLACE over S as bf16 hi | mid words (the A operand of the second product)
-//   O_h[128 q x 64 ch] = P_h V          A = P_h from tensor memory, B = the V tile [64 keys x 64 ch] as an MN-major
-//                                       128B-swizzled operand; only channels [16 h, 16 h + 16) of O_h belong to head h
-//                                       (the other 48 columns are the price of a descriptor convention that is pinned)
-//   acc_h = acc_h * corr + O_h          the softmax threads read their head's 16 columns and keep the running
-//                                       numerator in registers, so O never needs a rescale in tensor memory
-// At the end every CTA writes (m, l, acc[16]) per (query, head) -- flash-decoding partials -- and
+// CTA = (key split, query tile of 64, batch); 8 warps: warp w owns queries 16 (w & 3) .. + 15 and heads 4 (w >> 2) .. + 3.
+// Key tiles of 64 keys stream through a double-buffered cp.async ring (K planes | V planes, padded rows: conflict-free
+// fragment loads).  Per key tile and head:
+//   S_h[16 q x 64 keys] = Q_h K_h^T   six-term split product (lo hi, hi lo, mid mid, mid hi, hi mid, hi hi: error ~2^-26)
+//   P_h = exp(S_h - m)                online softmax, running maximum m and sum l per query row in registers; the S
+//                                     accumulator fragments ARE the A fragments of the next product (bf16 hi | mid)
+//   O_h = O_h * corr + P_h V_h        three-term split product; V fragments through ldmatrix.trans
+// At the end every warp writes (m, l, acc[16]) per (query, head) -- flash-decoding partials -- and
 // xattn_combine_kernel merges the key splits (one warp per (batch, head, query), lanes over the splits).
 #include "tc_common.cuh"
 
@@ -27,46 +22,22 @@ namespace {
 using namespace tc;
 
 constexpr int XT_KEYS = 64;                          // keys per tile
-constexpr int XT_BOX = XT_KEYS * 128;                // one K / V box: 64 rows x 128 B
-constexpr int XT_STAGE = 5 * XT_BOX;                 // K hi | K mid | K lo | V hi | V mid
-constexpr int XT_RING = 4;
-constexpr int XT_QBOX = 128 * 128;                   // 128 queries x 128 B
-constexpr int XT_Q_OFF = 0, XT_RING_OFF = 3 * XT_QBOX, XT_BAR_OFF = XT_RING_OFF + XT_RING * XT_STAGE;
-constexpr int XT_SMEM = XT_BAR_OFF + 256;
-constexpr int XT_THREADS = 10 * 32;                  // producer, MMA issuer, 8 softmax warps
+constexpr int XT_QT = 64;                            // queries per CTA
+constexpr int KSTR = 196, VSTR = 132;                // padded row strides (words) of the K (hi|mid|lo) and V (hi|mid) planes
+constexpr int XT_STAGE_WORDS = XT_KEYS * (KSTR + VSTR);
+constexpr int XT_Q_WORDS = XT_QT * KSTR;
+constexpr int XT_SMEM = (XT_Q_WORDS + 2 * XT_STAGE_WORDS) * 4;
+constexpr int XT_THREADS = 256;
 static_assert(XT_SMEM <= 232448, "xattn kernel exceeds the shared-memory limit");
 
-// kind::f16: bf16 x bf16 -> fp32, M = 128, N = 64.  S: A and B K-major.  PV: B MN-major (bit 16).
-constexpr uint32_t XIDESC_S = (1u << 4) | (1u << 7) | (1u << 10) | ((64u >> 3) << 17) | ((128u >> 4) << 24);
-constexpr uint32_t XIDESC_PV = XIDESC_S | (1u << 16);
-
-__device__ __forceinline__ void x_umma_ss(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc, uint32_t accumulate) {
+__device__ __forceinline__ void x_mma(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
   asm volatile(
-      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\ttcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}" ::"r"(
-          tmem_d),
-      "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "mma.sync.aligned.m16n8k16.row.col.f32.bf16.bf16.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
-__device__ __forceinline__ uint64_t x_desc_mn(uint32_t smem_addr, uint32_t lbo_bytes) {
-  return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | (64ull << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-__device__ __forceinline__ float x_ex2(float x) {
-  float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
-  return y;
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, float (&v)[16]) {
-  uint32_t r[16];
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]), "=r"(r[9]),
-        "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-  asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-  for (int i = 0; i < 16; ++i) v[i] = __uint_as_float(r[i]);
+__device__ __forceinline__ void x_cp16(uint32_t dst, const void* src, bool ok) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(src), "r"(ok ? 16 : 0) : "memory");
 }
 
 struct XtParams {
@@ -75,208 +46,169 @@ struct XtParams {
 };
 
 __global__ void __launch_bounds__(XT_THREADS, 1)
-xattn_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
-                const __grid_constant__ CUtensorMap mapV, const XtParams p) {
-  extern __shared__ __align__(1024) uint8_t smem_raw[];
-  const uint32_t base = smem_u32(smem_raw);
-  if ((base & 1023u) != 0u) __trap();
-  const uint32_t bars = base + XT_BAR_OFF;
-  const uint32_t q_full = bars, s_full = bars + 8, p_full = bars + 16, o_full = bars + 24, o_empty = bars + 32;
-  auto full = [&](int s) { return bars + 40u + 8u * s; };
-  auto empty = [&](int s) { return bars + 40u + 8u * XT_RING + 8u * s; };
-  const uint32_t tmem_slot = bars + 40u + 16u * XT_RING;
-  volatile uint32_t* tmem_slot_ptr = reinterpret_cast<volatile uint32_t*>(smem_raw + XT_BAR_OFF + 40 + 16 * XT_RING);
-
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int sp = blockIdx.x, mt = blockIdx.y >> 1, box = blockIdx.y & 1, b = blockIdx.z;
+xattn_tc_kernel(const uint32_t* __restrict__ qp, const uint32_t* __restrict__ kp, const uint32_t* __restrict__ vp,
+                const XtParams p) {
+  extern __shared__ __align__(16) uint32_t xs[];     // Q tile [64][KSTR] | 2 stages of K [64][KSTR], V [64][VSTR]
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int sp = blockIdx.x, mt = blockIdx.y, b = blockIdx.z;
   const int k_begin = sp * p.chunk, k_end = min(p.HW, k_begin + p.chunk);
   const int ntiles = (k_end - k_begin + XT_KEYS - 1) / XT_KEYS;          // >= 1 (the host sizes the splits)
+  const uint32_t sbase = smem_u32(xs);
 
-  if (warp == 0 && lane < 3) {
-    const CUtensorMap* mp = lane == 0 ? &mapQ : lane == 1 ? &mapK : &mapV;
-    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(mp)) : "memory");
+  // Q tile (rows past P are zero)
+  for (int i = tid; i < XT_QT * 48; i += XT_THREADS) {
+    const int r = i / 48, c4 = i % 48;
+    const int qi = mt * XT_QT + r;
+    const bool ok = qi < p.P;
+    x_cp16(sbase + (uint32_t)(r * KSTR + c4 * 4) * 4u, ok ? qp + ((size_t)b * p.P + qi) * 192 + c4 * 4 : qp, ok);
   }
-  if (threadIdx.x == 0) {
-    mbar_init(q_full, 1);
-    mbar_init(s_full, 1);
-    mbar_init(p_full, 8);
-    mbar_init(o_full, 1);
-    mbar_init(o_empty, 8);
-    for (int s = 0; s < XT_RING; ++s) {
-      mbar_init(full(s), 1);
-      mbar_init(empty(s), 1);
+  auto issue = [&](int i) {
+    const uint32_t st = sbase + (uint32_t)(XT_Q_WORDS + (i & 1) * XT_STAGE_WORDS) * 4u;
+    const int row0 = k_begin + i * XT_KEYS;
+    for (int j = tid; j < XT_KEYS * 80; j += XT_THREADS) {
+      const int r = j / 80, c4 = j % 80;
+      const int key = row0 + r;
+      const bool ok = key < k_end;
+      const size_t grow = (size_t)b * p.HW + key;
+      if (c4 < 48) x_cp16(st + (uint32_t)(r * KSTR + c4 * 4) * 4u, ok ? kp + grow * 192 + c4 * 4 : kp, ok);
+      else x_cp16(st + (uint32_t)(XT_KEYS * KSTR + r * VSTR + (c4 - 48) * 4) * 4u, ok ? vp + grow * 128 + (c4 - 48) * 4 : vp, ok);
     }
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 1) {
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(tmem_slot), "r"(512u) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  tc_fence_before();
-  __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot_ptr;
+    asm volatile("cp.async.commit_group;" ::: "memory");
+  };
 
-  if (warp == 0) {
-    // ---------------- TMA producer ----------------
-    if (lane == 0) {
-      const int q0 = b * p.P + mt * 128;
-      mbar_expect_tx(q_full, 3 * XT_QBOX);
+  const int q0 = 16 * (warp & 3), h0 = 4 * (warp >> 2);
+  constexpr float L2E = 1.4426950408889634f;
+  float m[4][2], l[4][2], acc[4][2][4];
 #pragma unroll
-      for (int pl = 0; pl < 3; ++pl)                                                 // hi, mid, lo planes
-        tma_load_2d(base + XT_Q_OFF + pl * XT_QBOX, &mapQ, q_full, 128 * pl + 64 * box, q0);
-      for (int i = 0; i < ntiles; ++i) {
-        const int s = i % XT_RING;
-        if (i >= XT_RING) mbar_wait(empty(s), ((i / XT_RING) - 1) & 1);
-        const uint32_t st = base + XT_RING_OFF + s * XT_STAGE;
-        const int row = b * p.HW + k_begin + i * XT_KEYS;
-        mbar_expect_tx(full(s), XT_STAGE);
+  for (int h = 0; h < 4; ++h) {
+    m[h][0] = m[h][1] = -INFINITY;
+    l[h][0] = l[h][1] = 0.f;
 #pragma unroll
-        for (int pl = 0; pl < 3; ++pl) tma_load_2d(st + pl * XT_BOX, &mapK, full(s), 128 * pl + 64 * box, row);
-        tma_load_2d(st + 3 * XT_BOX, &mapV, full(s), 64 * box, row);
-        tma_load_2d(st + 4 * XT_BOX, &mapV, full(s), 128 + 64 * box, row);
-      }
-    }
-  } else if (warp == 1) {
-    // ---------------- MMA issuer ----------------
-    const uint32_t qb = base + XT_Q_OFF;
-    mbar_wait(q_full, 0);
-    for (int i = 0; i < ntiles; ++i) {
-      const int s = i % XT_RING;
-      mbar_wait(full(s), (i / XT_RING) & 1);
-      tc_fence_after();
-      const uint32_t kb = base + XT_RING_OFF + s * XT_STAGE;
-      if (elect_one()) {
-#pragma unroll
-        for (int hh = 0; hh < 4; ++hh) {
-          const uint64_t q_hi = umma_desc(qb + hh * 32), q_mid = umma_desc(qb + XT_QBOX + hh * 32),
-                         q_lo = umma_desc(qb + 2 * XT_QBOX + hh * 32);
-          const uint64_t k_hi = umma_desc(kb + hh * 32), k_mid = umma_desc(kb + XT_BOX + hh * 32),
-                         k_lo = umma_desc(kb + 2 * XT_BOX + hh * 32);
-          const uint32_t d = tmem_base + (uint32_t)(64 * hh);
-          x_umma_ss(d, q_lo, k_hi, XIDESC_S, 0);              // smallest terms first
-          x_umma_ss(d, q_hi, k_lo, XIDESC_S, 1);
-          x_umma_ss(d, q_mid, k_mid, XIDESC_S, 1);
-          x_umma_ss(d, q_mid, k_hi, XIDESC_S, 1);
-          x_umma_ss(d, q_hi, k_mid, XIDESC_S, 1);
-          x_umma_ss(d, q_hi, k_hi, XIDESC_S, 1);
-        }
-        umma_commit(s_full);
-      }
-      __syncwarp();
-      mbar_wait(p_full, i & 1);                             // P of this tile is in tensor memory
-      if (i > 0) mbar_wait(o_empty, (i - 1) & 1);           // the previous tile's O columns have been read
-      tc_fence_after();
-      if (elect_one()) {
-        const uint32_t vb = kb + 3 * XT_BOX;
-#pragma unroll
-        for (int hh = 0; hh < 4; ++hh) {
-          const uint32_t d = tmem_base + 256u + (uint32_t)(64 * hh);
-#pragma unroll
-          for (int t = 0; t < XT_KEYS / 16; ++t) {
-            const uint64_t v_hi = x_desc_mn(vb + t * 2048, XT_BOX), v_mid = x_desc_mn(vb + XT_BOX + t * 2048, XT_BOX);
-            const uint32_t p_hi = tmem_base + (uint32_t)(64 * hh + 16 * t), p_mid = p_hi + 8u;
-            umma_bf16_ts(d, p_mid, v_hi, XIDESC_PV, t != 0);
-            umma_bf16_ts(d, p_hi, v_mid, XIDESC_PV, 1);
-            umma_bf16_ts(d, p_hi, v_hi, XIDESC_PV, 1);
-          }
-        }
-        umma_commit(empty(s));
-        umma_commit(o_full);
-      }
-      __syncwarp();
-    }
-  } else {
-    // ---------------- softmax / accumulation (warps 2..9): thread = query = TMEM lane, two heads per warp ----------------
-    const int qd = warp & 3, sub = (warp - 2) >> 2;
-    const int qrow = mt * 128 + qd * 32 + lane;            // query index inside the sample
-    const uint32_t tlane = tmem_base + ((uint32_t)(qd * 32) << 16);
-    constexpr float L2E = 1.4426950408889634f;
-    float m[2] = {-INFINITY, -INFINITY}, l[2] = {0.f, 0.f}, acc[2][16], corr[2];
-#pragma unroll
-    for (int h2 = 0; h2 < 2; ++h2)
-#pragma unroll
-      for (int c = 0; c < 16; ++c) acc[h2][c] = 0.f;
-    for (int i = 0; i < ntiles; ++i) {
-      const int nvalid = min(XT_KEYS, k_end - (k_begin + i * XT_KEYS));
-      mbar_wait(s_full, i & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int h2 = 0; h2 < 2; ++h2) {
-        const int hh = 2 * sub + h2;
-        float v[2][32];
-        tmem_ld32_nowait(tlane + (uint32_t)(64 * hh), v[0]);
-        tmem_ld32_nowait(tlane + (uint32_t)(64 * hh + 32), v[1]);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        float mx = -INFINITY;
-#pragma unroll
-        for (int u = 0; u < 2; ++u)
-#pragma unroll
-          for (int j = 0; j < 32; ++j)
-            if (u * 32 + j < nvalid) mx = fmaxf(mx, v[u][j]);
-        const float mn = fmaxf(m[h2], mx);
-        corr[h2] = x_ex2((m[h2] - mn) * L2E);              // exp2(-inf) = 0 on the first tile
-        const float mc = mn * L2E;
-        float sum = 0.f;
-#pragma unroll
-        for (int u = 0; u < 2; ++u) {
-#pragma unroll
-          for (int j = 0; j < 32; ++j) {
-            v[u][j] = (u * 32 + j < nvalid) ? x_ex2(fmaf(v[u][j], L2E, -mc)) : 0.f;
-            sum += v[u][j];
-          }
-          // two k-steps (16 keys each): 8 words of bf16 hi pairs | 8 words of mid pairs
-          uint32_t w[32];
-#pragma unroll
-          for (int t = 0; t < 2; ++t)
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              const float a = v[u][16 * t + 2 * j], bb = v[u][16 * t + 2 * j + 1];
-              const uint32_t hi = pack_bf16x2(a, bb);
-              w[16 * t + j] = hi;
-              w[16 * t + 8 + j] = pack_bf16x2(a - __uint_as_float(hi << 16), bb - __uint_as_float(hi & 0xFFFF0000u));
-            }
-          tmem_st32(tlane + (uint32_t)(64 * hh + 32 * u), w);
-        }
-        l[h2] = l[h2] * corr[h2] + sum;
-        m[h2] = mn;
-      }
-      asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory");
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(p_full);
-      // numerator of this tile: the head's 16 channels of O
-      mbar_wait(o_full, i & 1);
-      tc_fence_after();
-#pragma unroll
-      for (int h2 = 0; h2 < 2; ++h2) {
-        const int hh = 2 * sub + h2;
-        float o[16];
-        tmem_ld16(tlane + 256u + (uint32_t)(64 * hh + 16 * hh), o);
-#pragma unroll
-        for (int c = 0; c < 16; ++c) acc[h2][c] = fmaf(acc[h2][c], corr[h2], o[c]);
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(o_empty);
-    }
-    if (qrow < p.P) {
-#pragma unroll
-      for (int h2 = 0; h2 < 2; ++h2) {
-        const int head = 4 * box + 2 * sub + h2;
-        float* pp = p.part + (((size_t)(b * p.heads + head) * p.nsplit + sp) * 18) * p.P + qrow;
-        pp[0] = m[h2];
-        pp[p.P] = l[h2];
-#pragma unroll
-        for (int c = 0; c < 16; ++c) pp[(size_t)(2 + c) * p.P] = acc[h2][c];
-      }
-    }
+    for (int cb = 0; cb < 2; ++cb) acc[h][cb][0] = acc[h][cb][1] = acc[h][cb][2] = acc[h][cb][3] = 0.f;
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(512u) : "memory");
+
+  issue(0);
+  for (int i = 0; i < ntiles; ++i) {
+    if (i + 1 < ntiles) {
+      issue(i + 1);
+      asm volatile("cp.async.wait_group 1;" ::: "memory");
+    } else {
+      asm volatile("cp.async.wait_group 0;" ::: "memory");
+    }
+    __syncthreads();
+    const int nvalid = min(XT_KEYS, k_end - (k_begin + i * XT_KEYS));
+    const uint32_t* ks = xs + XT_Q_WORDS + (i & 1) * XT_STAGE_WORDS;
+    const uint32_t vs_addr = sbase + (uint32_t)(XT_Q_WORDS + (i & 1) * XT_STAGE_WORDS + XT_KEYS * KSTR) * 4u;
+#pragma unroll
+    for (int hh = 0; hh < 4; ++hh) {                  // unrolled: the per-head state stays in registers
+      const int h = h0 + hh;
+      // Q fragments of this head: planes hi (0), mid (64), lo (128); channel pair words 8h + t (+4)
+      uint32_t qa[3][4];
+#pragma unroll
+      for (int pl = 0; pl < 3; ++pl) {
+        const uint32_t* qr0 = xs + (q0 + g) * KSTR + 64 * pl + 8 * h + t;
+        const uint32_t* qr1 = qr0 + 8 * KSTR;
+        qa[pl][0] = qr0[0]; qa[pl][1] = qr1[0]; qa[pl][2] = qr0[4]; qa[pl][3] = qr1[4];
+      }
+      float S[8][4];
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb) {
+        S[nb][0] = S[nb][1] = S[nb][2] = S[nb][3] = 0.f;
+        const uint32_t* kr = ks + (nb * 8 + g) * KSTR + 8 * h + t;
+        const uint32_t khi0 = kr[0], khi1 = kr[4], kmid0 = kr[64], kmid1 = kr[68], klo0 = kr[128], klo1 = kr[132];
+        x_mma(S[nb], qa[2], khi0, khi1);            // smallest terms first
+        x_mma(S[nb], qa[0], klo0, klo1);
+        x_mma(S[nb], qa[1], kmid0, kmid1);
+        x_mma(S[nb], qa[1], khi0, khi1);
+        x_mma(S[nb], qa[0], kmid0, kmid1);
+        x_mma(S[nb], qa[0], khi0, khi1);
+      }
+      // online softmax: rows g (j = 0, 1) and g + 8 (j = 2, 3); key of element j = nb * 8 + 2t + (j & 1)
+      float mx[2] = {-INFINITY, -INFINITY};
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          if (nb * 8 + 2 * t + (j & 1) >= nvalid) S[nb][j] = -INFINITY;
+          mx[j >> 1] = fmaxf(mx[j >> 1], S[nb][j]);
+        }
+      float corr[2], mc[2];
+#pragma unroll
+      for (int r = 0; r < 2; ++r) {
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 1));
+        mx[r] = fmaxf(mx[r], __shfl_xor_sync(0xffffffffu, mx[r], 2));
+        const float mn = fmaxf(m[hh][r], mx[r]);
+        corr[r] = exp2f((m[hh][r] - mn) * L2E);     // 0 on the first tile (m = -inf)
+        mc[r] = mn * L2E;
+        m[hh][r] = mn;
+      }
+      float sum[2] = {0.f, 0.f};
+#pragma unroll
+      for (int nb = 0; nb < 8; ++nb)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) {
+          S[nb][j] = exp2f(fmaf(S[nb][j], L2E, -mc[j >> 1]));   // exp2(-inf) = 0 for keys past the end
+          sum[j >> 1] += S[nb][j];
+        }
+#pragma unroll
+      for (int r = 0; r < 2; ++r) l[hh][r] = l[hh][r] * corr[r] + sum[r];
+#pragma unroll
+      for (int cb = 0; cb < 2; ++cb)
+#pragma unroll
+        for (int j = 0; j < 4; ++j) acc[hh][cb][j] *= corr[j >> 1];
+      // O += P V: k-step kt = keys 16 kt .. + 15 (S blocks 2 kt, 2 kt + 1)
+#pragma unroll
+      for (int kt = 0; kt < 4; ++kt) {
+        uint32_t ph[4], pm[4];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const float* sv = S[2 * kt + (e >> 1)] + 2 * (e & 1);
+          const uint32_t hw = pack_bf16x2(sv[0], sv[1]);
+          ph[e] = hw;
+          pm[e] = pack_bf16x2(sv[0] - __uint_as_float(hw << 16), sv[1] - __uint_as_float(hw & 0xFFFF0000u));
+        }
+#pragma unroll
+        for (int cb = 0; cb < 2; ++cb) {
+          // matrices: keys 0-7 hi, keys 8-15 hi, keys 0-7 mid, keys 8-15 mid of channels 16 h + 8 cb .. + 7
+          const int key = 16 * kt + (lane & 7) + ((lane >> 3) & 1) * 8;
+          const uint32_t addr = vs_addr + (uint32_t)(key * VSTR + (lane >> 4) * 64 + 8 * h + 4 * cb) * 4u;
+          uint32_t vh0, vh1, vm0, vm1;
+          asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(vh0), "=r"(vh1), "=r"(vm0), "=r"(vm1)
+                       : "r"(addr));
+          x_mma(acc[hh][cb], pm, vh0, vh1);
+          x_mma(acc[hh][cb], ph, vm0, vm1);
+          x_mma(acc[hh][cb], ph, vh0, vh1);
+        }
+      }
+    }
+    __syncthreads();                                   // stage (i & 1) is refilled by the next issue
+  }
+  // partials of rows g, g + 8: (m, l, 16 channels)
+#pragma unroll
+  for (int hh = 0; hh < 4; ++hh) {
+    const int head = h0 + hh;
+#pragma unroll
+    for (int r = 0; r < 2; ++r) {
+      float lr = l[hh][r];
+      lr += __shfl_xor_sync(0xffffffffu, lr, 1);
+      lr += __shfl_xor_sync(0xffffffffu, lr, 2);
+      const int qi = mt * XT_QT + q0 + g + 8 * r;
+      if (qi < p.P) {
+        float* pp = p.part + (((size_t)(b * p.heads + head) * p.nsplit + sp) * 18) * p.P + qi;
+        if (t == 0) {
+          pp[0] = m[hh][r];
+          pp[p.P] = lr;
+        }
+#pragma unroll
+        for (int cb = 0; cb < 2; ++cb) {
+          const int c = 8 * cb + 2 * t;
+          pp[(size_t)(2 + c) * p.P] = acc[hh][cb][2 * r];
+          pp[(size_t)(3 + c) * p.P] = acc[hh][cb][2 * r + 1];
+        }
+      }
+    }
   }
 }
 
@@ -348,25 +280,13 @@ __global__ void kv_planes_kernel(const float* __restrict__ kv, int ld, uint32_t*
   }
 }
 
-bool make_rows_map(CUtensorMap* m, const void* ptr, long long rows, int ld_words, int box_rows) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[2] = {(cuuint64_t)ld_words * 2, (cuuint64_t)rows};
-  cuuint64_t strides[1] = {(cuuint64_t)ld_words * 4};
-  cuuint32_t box[2] = {64, (cuuint32_t)box_rows};
-  cuuint32_t estr[2] = {1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 2, const_cast<void*>(ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 bool g_xt_attr[64];
 
 }  // namespace
 
 extern "C" {
 
-// Operand planes of the tcgen05 cross attention.  q [M, ld] fp32 (128 channels, pre-scaled) -> qplanes [M, 192 words]
+// Operand planes of the tensor-core cross attention.  q [M, ld] fp32 (128 channels, pre-scaled) -> qplanes [M, 192 words]
 // (bf16 hi | mid | lo); kv [Mk, ld_kv >= 256] fp32 (K | V) -> kplanes [Mk, 192 words], vplanes [Mk, 128 words] (hi | mid).
 int di_attn_planes_f32(const float* q, int ld_q, void* qplanes, int M, const float* kv, int ld_kv, void* kplanes,
                        void* vplanes, long long Mk, cudaStream_t stream) {
@@ -382,7 +302,13 @@ int di_attn_planes_f32(const float* q, int ld_q, void* qplanes, int M, const flo
 
 // Number of key splits di_xattn_tc_f32 uses for (B, HW): the caller sizes `part` as B * heads * nsplit * 18 * P floats.
 int di_xattn_tc_splits(int B, int HW) {
-  int n = 148 / (4 * (B > 0 ? B : 1));
+  int dev = 0, sms = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess ||
+      sms <= 0) {
+    di_set_error("di_xattn_tc_splits: cannot query the SM count");
+    return DI_ERR_LAUNCH;
+  }
+  int n = sms / (2 * (B > 0 ? B : 1));              // with the 4 query tiles of P = 200: two CTAs' worth of work per SM
   if (n < 1) n = 1;
   const int tiles = (HW + XT_KEYS - 1) / XT_KEYS;
   if (n > tiles) n = tiles;
@@ -414,20 +340,17 @@ int di_xattn_tc_f32(const void* q, const void* k, const void* v, float* part, fl
     }
     g_xt_attr[devid] = true;
   }
-  CUtensorMap mq, mk, mv;
-  if (!(make_rows_map(&mq, q, (long long)B * P, 192, 128) && make_rows_map(&mk, k, (long long)B * HW, 192, XT_KEYS) &&
-        make_rows_map(&mv, v, (long long)B * HW, 128, XT_KEYS))) {
-    di_set_error("di_xattn_tc_f32: cuTensorMapEncodeTiled failed");
-    return DI_ERR_LAUNCH;
-  }
   XtParams p{};
   p.P = P; p.HW = HW; p.heads = heads;
   p.nsplit = di_xattn_tc_splits(B, HW);
+  if (p.nsplit < 0) return p.nsplit;
   const int tiles = (HW + XT_KEYS - 1) / XT_KEYS;
   p.chunk = ((tiles + p.nsplit - 1) / p.nsplit) * XT_KEYS;
   p.part = part;
-  const int mtiles = (P + 127) / 128;
-  xattn_tc_kernel<<<dim3(p.nsplit, 2 * mtiles, B), XT_THREADS, XT_SMEM, stream>>>(mq, mk, mv, p);
+  const int mtiles = (P + XT_QT - 1) / XT_QT;
+  xattn_tc_kernel<<<dim3(p.nsplit, mtiles, B), XT_THREADS, XT_SMEM, stream>>>(static_cast<const uint32_t*>(q),
+                                                                            static_cast<const uint32_t*>(k),
+                                                                            static_cast<const uint32_t*>(v), p);
   DI_CHECK_LAUNCH("di_xattn_tc_f32");
   xattn_combine_kernel<<<di_cdiv((long long)B * heads * P, 8), 256, 0, stream>>>(part, out, B, P, heads * 16, heads, p.nsplit);
   DI_CHECK_LAUNCH("di_xattn_tc_f32 (combine)");

@@ -130,10 +130,10 @@ def split_bf16(w):
 
 
 def split_rows(x, kind):
-    """Host model of the pre-split operand format of the window kernel (gemm_tc.cu split_block): x [M, C] fp32 ->
+    """Host model of the pre-split operand format of the window kernel (gemm_tc.cu epilogue): x [M, C] fp32 ->
     [M, C] fp32-typed tensor whose 32-bit words are packed bf16x2 (hi = bf16(x), mid = bf16(x - hi), lower channel in
     the low half).  kind 1: channel pair j -> words 2j (hi), 2j+1 (mid); kind 2: channel group of 8 -> 4 hi | 4 mid;
-    kind 3 (planar, tcgen05 window kernel): channel group of 128 -> 64 hi words | 64 mid words."""
+    kind 3 (planar window kernel): channel group of 128 -> 64 hi words | 64 mid words."""
     x = x.to(torch.float32)
     hi = x.to(torch.bfloat16)
     mid = (x - hi.to(torch.float32)).to(torch.bfloat16)
@@ -156,7 +156,7 @@ def split_rows(x, kind):
 
 class Weight:
     """A dense-layer weight [N, K] kept in the forms the kernels consume: plain fp32 (FFMA path), the TF32 hi/lo
-    split and the bf16 hi/mid split (tcgen05 paths)."""
+    split and the bf16 hi/mid split (tensor-core paths)."""
 
     def __init__(self, w, device, lazy=False):
         """lazy: build the two splits on first use (training: weights change every step and only one split is read)."""

@@ -1,7 +1,7 @@
 """CUDA-graph replay of a fixed kernel schedule.
 
-One forward of the MMRI+MMPI path is ~140 kernel launches; issued from Python they cost ~5 ms of host time per
-frame, as much as the GPU work itself.  The schedule has no data-dependent host control flow, so it can be
+One forward of the MMRI+MMPI path is ~140 kernel launches; issued from Python their host cost per frame is of the
+order of the GPU work itself.  The schedule has no data-dependent host control flow, so it can be
 captured once per input signature (shapes incl. pillar / point counts) and replayed: per frame the host only
 copies the small camera constants and calls cudaGraphLaunch.
 

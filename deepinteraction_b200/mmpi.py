@@ -6,7 +6,7 @@ Reference: projects/mmdet3d_plugin/models/dense_heads/deepinteraction_decoder.py
 :35-113, MultiheadAttention :116-495, FFN :498-581, DynamicConv :584-629, ImageRCNNBlock :632-761,
 PointRCNNBlock :765-841), core/bbox/coders/transfusion_bbox_coder.py.
 
-B200-first differences from the reference schedule (results unchanged, fp32):
+Differences from the reference schedule (results unchanged, fp32):
   * queries are rows [B*P, C]; maps are pixel-major, so the top-k gather, RoIAlign and the cross
     attention read contiguous 512-byte rows;
   * the key positional embedding of the query x BEV cross attention depends only on the BEV grid, so
@@ -468,7 +468,7 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         w_kv, b_kv, ckv = pk['cross_kv']
         kv = ops.linear([pts_conv.view(B * HW, C)], w_kv, b_kv, res=ckv, res_mod=HW)
         if ops.can_xattn_tc(P, C, H, B * HW):
-            a = ops.xattn_tc(qc, kv, B, P, HW, H)                   # tcgen05 attention kernel (xattn_tc.cu)
+            a = ops.xattn_tc(qc, kv, B, P, HW, H)                   # tensor-core attention kernel (xattn_tc.cu)
         else:
             a = ops.cross_attn(qc, kv, B, P, HW, H)
         q = self._mlp([a], *pk['cross_out'], res=q, ln=pk['norm2'])

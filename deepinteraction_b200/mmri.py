@@ -5,7 +5,7 @@ Reference: projects/mmdet3d_plugin/models/necks/deepinteraction_encoder.py:8-85 
 models/utils/encoder_utils.py (ConvBNReLU :11-34, LocalContextAttentionBlock :84-135, BEVWarp
 :137-199, MMRI_P2I :202-213, MMRI_I2P :216-320).
 
-B200-first differences from the reference schedule (results are unchanged, fp32):
+Differences from the reference schedule (results are unchanged, fp32):
   * feature maps live pixel-major (NHWC) between kernels; the NCHW inputs are consumed directly by
     the first 3x3 conv and the outputs are returned as NCHW-shaped channels-last views;
   * BatchNorm (eval) is folded into the 1x1 convs; each `cat + Conv+BN` pair is ONE 3-source GEMM;
@@ -116,9 +116,9 @@ def lcab_forward(pk, target, source, N, H, W):
     directly (bf16 hi/mid words, ops.linear_split), so the window kernel has no conversion work."""
     C = pk['C']
     pre = ops.can_presplit(N * H * W, C, pk['ks'])
-    tc = ops.can_window_tc(N * H * W, C, pk['ks'])       # tcgen05 window kernel: planar operands (split kind 3)
+    tc = ops.can_window_tc(N * H * W, C, pk['ks'])       # planar window kernel: planar operands (split kind 3)
     if tc and ops.LCAB_PROJ[0] and target.is_contiguous() and source.is_contiguous():
-        # one C-ABI call: all five projections in one launch (q1 / k1 stay on chip, lcab_proj.cu), then the window kernel
+        # one C-ABI call: the five projections (lcab_proj.cu), then the window kernel
         return ops.lcab_forward_tc(target, source, pk['w_self'], pk['b_self'], pk['w_2'], pk['b_2'], N, H, W)
     if target is source:
         if pre:

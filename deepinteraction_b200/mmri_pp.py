@@ -7,7 +7,7 @@ FFN, BaseTransformerLayer; SURVEY.md Appendix C.4 / C.5).  Parameter names equal
 loads unchanged (`img_fusion_blocks.N.attentions.M...`, `...ffns.K.layers.0.0`, `...norms.J`, `...scale`).
 
 Schedule (pixel-major rows, fp32; no torch math on device tensors):
-  * the three 3x3 convs on the tcgen05 implicit-GEMM kernel; per layer and modality
+  * the three 3x3 convs on the wgmma implicit-GEMM kernel; per layer and modality
     value_proj / (sampling_offsets | attention_weights) / output_proj / FFN as tensor-core GEMMs (the two query-side
     Linear layers are ONE GEMM), di_msdeform_f32 for the sampling core, LayerNorm + residual in di_rows_finish_f32;
   * MMRI_P2I: the BEVWarp geometry of the base encoder (depth scatter, GPU depth completion, lifting: once per frame)

@@ -15,9 +15,9 @@ from .fold import Weight
 ACT_NONE, ACT_RELU, ACT_GELU = 0, 1, 2
 
 LAUNCHES = [0]   # number of libdi_b200 kernel-launching calls (bench.py reports it)
-USE_TC = [os.environ.get('DI_B200_TC', '1') != '0']   # tcgen05 split-product path for Weight objects (else FFMA)
+USE_TC = [os.environ.get('DI_B200_TC', '1') != '0']   # wgmma split-product path for Weight objects (else FFMA)
 TC_CONV = [os.environ.get('DI_B200_TC_CONV', '1') != '0']
-TC_MIN_M = [int(os.environ.get('DI_B200_TC_MIN_M', '128'))]   # fewer rows: fp32 FFMA kernels of gemm.cu (measured: the tensor-core kernel is faster from 128 rows up)
+TC_MIN_M = [int(os.environ.get('DI_B200_TC_MIN_M', '128'))]   # fewer rows: fp32 FFMA kernels of gemm.cu (threshold not re-measured on the H100)
 TC_BF16 = [os.environ.get('DI_B200_TC_BF16', '1') != '0']   # bf16-split operands where K % 64 == 0 (else 3xTF32)
 _TAG = ['']        # optional shape tag for the next profiled call (bench.py --shapes table)
 PROFILE = [None]   # bench.py sets PROFILE[0] = [] to record (name, start_event, end_event, bytes, flops, module) per call
@@ -146,8 +146,8 @@ def _linear_tc(srcs, W, bias, act, out, res, res_mod, M, N, K):
 if os.environ.get('DI_B200_TC_SMS'):
     _lib.check(_lib.lib().di_tc_set_sm_limit(int(os.environ['DI_B200_TC_SMS'])), 'di_tc_set_sm_limit')
 
-# shared convs read the NCHW boundary tensors in place (no transposition pass).  Measured on B200: image conv
-# 251 us vs 208 + 65 us (transposition), BEV conv 204 us vs 111 + 39 us -> a wash overall, off by default.
+# shared convs read the NCHW boundary tensors in place (no transposition pass); off by default (not measured on the
+# H100).
 NCHW_DIRECT = [os.environ.get('DI_B200_NCHW_DIRECT', '0') != '0']
 PRESPLIT = [os.environ.get('DI_B200_PRESPLIT', '1') != '0']   # q/k/v projections emit bf16 (hi, mid) words for the window kernel
 
@@ -179,16 +179,16 @@ def linear_split(srcs, W, bias, act, split_col0, split_kind):
     return out
 
 
-WINDOW_TC = [os.environ.get('DI_B200_WINDOW_TC', '1') != '0']   # tcgen05 window kernel (C == 128) instead of mma.sync
+WINDOW_TC = [os.environ.get('DI_B200_WINDOW_TC', '1') != '0']   # planar-operand window kernel (C == 128) instead of the interleaved one
 
 
 def can_window_tc(M, C, ksize):
-    """True when the LCAB projections may emit planar operands for the tcgen05 window kernel (lcab_tc.cu)."""
+    """True when the LCAB projections may emit planar operands for the planar window kernel (lcab.cu)."""
     return bool(WINDOW_TC[0] and can_presplit(M, C, ksize) and C == 128)
 
 
 def lcab_window_tc(q, k, v, N, H, W, C, out=None):
-    """9x9 window attention on tcgen05 for planar pre-split q, k, v row views (linear_split kind 3)."""
+    """9x9 window attention for planar pre-split q, k, v row views (linear_split kind 3)."""
     if out is None:
         out = torch.empty(N * H * W, C, device=q.device, dtype=torch.float32)
     (pq, lq), (pk, lk), (pv, lv), (po, lo) = _rows(q), _rows(k), _rows(v), _rows(out)
@@ -197,11 +197,11 @@ def lcab_window_tc(q, k, v, N, H, W, C, out=None):
     return out
 
 
-LCAB_PROJ = [os.environ.get('DI_B200_LCAB_PROJ', '1') != '0']   # fused projection chain (lcab_proj.cu) in front of the tcgen05 window kernel
+LCAB_PROJ = [os.environ.get('DI_B200_LCAB_PROJ', '1') != '0']   # projection chain (lcab_proj.cu) in front of the planar window kernel
 
 
 def lcab_proj(x_t, x_s, w1, b1, w2, b2):
-    """q, k, v (planar operands of lcab_window_tc) from the target / source rows in ONE launch: w1 = Weight of
+    """q, k, v (planar operands of lcab_window_tc) from the target / source rows in one call (five GEMM launches): w1 = Weight of
     [q1 | k1 | v] (384 x 128), w2 = Weight of [q2 | k2] (256 x 128), BN folded."""
     M = x_t.shape[0]
     assert x_t.shape[1] == 128 and x_s.shape == x_t.shape and w1.shape == (384, 128) and w2.shape == (256, 128)
@@ -209,12 +209,12 @@ def lcab_proj(x_t, x_s, w1, b1, w2, b2):
     (pt, lt), (ps, ls) = _rows(x_t), _rows(x_s)
     _call('di_lcab_proj_f32', pt, lt, ps, ls, _ptr(w1.bh), _ptr(w1.bm), _ptr(b1), _ptr(w2.bh), _ptr(w2.bm), _ptr(b2),
           _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), M, _stream(),
-          nbytes=4 * M * 128 * (4 if x_t is x_s else 5), flops=2 * 5 * M * 128 * 128)
+          nbytes=4 * M * 128 * (4 if x_t is x_s else 5), flops=2 * 5 * M * 128 * 128, launches=5)
     return out[0], out[1], out[2]
 
 
 def lcab_forward_tc(x_t, x_s, w1, b1, w2, b2, N, H, W):
-    """LocalContextAttentionBlock for C = 128 in one C-ABI call (projection chain + tcgen05 window kernel).  The byte count
+    """LocalContextAttentionBlock for C = 128 in one C-ABI call (projection chain + planar window kernel).  The byte count
     is the MODULE-boundary one of SURVEY.md 8(d): each distinct input map read once, the output written once."""
     M = x_t.shape[0]
     assert M == N * H * W and x_t.shape[1] == 128 and x_s.shape == x_t.shape
@@ -223,7 +223,7 @@ def lcab_forward_tc(x_t, x_s, w1, b1, w2, b2, N, H, W):
     (pt, lt), (ps, ls) = _rows(x_t), _rows(x_s)
     _call('di_lcab_forward_f32', pt, lt, ps, ls, _ptr(w1.bh), _ptr(w1.bm), _ptr(b1), _ptr(w2.bh), _ptr(w2.bm), _ptr(b2),
           _ptr(qkv), _ptr(out), 128, N, H, W, _stream(),
-          nbytes=4 * M * 128 * (2 if x_t is x_s else 3), flops=2 * 5 * M * 128 * 128 + 2 * 2 * 81 * M * 128, launches=2)
+          nbytes=4 * M * 128 * (2 if x_t is x_s else 3), flops=2 * 5 * M * 128 * 128 + 2 * 2 * 81 * M * 128, launches=6)
     return out
 
 
@@ -819,8 +819,8 @@ def bev_sample_bwd(d_out, grid, V, bev_shape):
     return d_bev
 
 
-# ---- tcgen05 query x BEV cross attention (csrc/xattn_tc.cu) ----------------------------------------------------------
-XATTN_TC = [os.environ.get('DI_B200_XATTN_TC', '1') != '0']   # tcgen05 query x BEV cross attention (xattn_tc.cu)
+# ---- tensor-core query x BEV cross attention (csrc/xattn_tc.cu) ----------------------------------------------------------
+XATTN_TC = [os.environ.get('DI_B200_XATTN_TC', '1') != '0']   # tensor-core query x BEV cross attention (xattn_tc.cu)
 
 
 def can_xattn_tc(P, C, heads, M_keys):
@@ -829,7 +829,7 @@ def can_xattn_tc(P, C, heads, M_keys):
 
 def xattn_tc(q, kv, B, P, HW, heads):
     """q [B*P, 128] fp32 (pre-scaled queries), kv [B*HW, 256] fp32 (K | V) -> softmax(q k^T) v per head, [B*P, 128] fp32:
-    operand planes (di_attn_planes_f32) + the tcgen05 attention kernel + the split merge."""
+    operand planes (di_attn_planes_f32) + the mma.sync attention kernel + the split merge."""
     assert kv.is_contiguous() and kv.shape == (B * HW, 256) and q.shape == (B * P, 128)
     dev_ = q.device
     qp = torch.empty(B * P, 192, device=dev_, dtype=torch.float32)

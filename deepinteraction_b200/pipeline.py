@@ -13,17 +13,15 @@ from . import _lib
 
 class FramePipeline:
     def __init__(self, neck, head, depth=3, device=None, tc_sms=140):
-        """depth: frames in flight (measured on B200, base model: 1 -> 219, 2 -> 272, 3 -> 300, 4 -> 307 frames/s).
+        """depth: frames in flight.
         tc_sms: with depth > 1 the persistent tensor-core grids are capped at this many CTAs so that the other frames'
-        small decoder kernels always find a free SM (process-wide setting of libdi_b200, ~3 %; 0 = leave as is)."""
+        small decoder kernels always find a free SM (process-wide setting of libdi_b200; 0 = leave as is)."""
         self.neck, self.head, self.depth = neck, head, depth
         self.streams = [torch.cuda.Stream(device=device) for _ in range(depth)]
         self.count = 0
         if depth > 1 and tc_sms:
             L = _lib.lib()
             _lib.check(L.di_tc_set_sm_limit(int(tc_sms)), 'di_tc_set_sm_limit')
-            _lib.check(L.di_lcab_window_tc_set_sm_limit(int(tc_sms)), 'di_lcab_window_tc_set_sm_limit')
-            _lib.check(L.di_lcab_proj_set_sm_limit(int(tc_sms)), 'di_lcab_proj_set_sm_limit')
 
     def submit(self, frame, wait_event=None, stream_index=None):
         """frame: dict(img_feats, pts_feats, img_metas, pts_metas) of device tensors.  Returns (out, done_event,

@@ -6,7 +6,7 @@ Reference: models/necks/deepinteraction_encoder.py:8-85 run under `model.train()
 through them; the gradient of the whole model is then all-reduced (tools/train.py:157 -> shard.GradBuckets here).
 
 Eval-mode BatchNorm folds into the 1x1 convolutions (the inference kernels; backward.py differentiates that form).
-Batch statistics depend on the data, so this path keeps the layers apart: raw 1x1 product on the tcgen05 / FFMA GEMMs
+Batch statistics depend on the data, so this path keeps the layers apart: raw 1x1 product on the wgmma / FFMA GEMMs
 (3xTF32 split), column moments (di_bn_stats_f32), normalise + ReLU (di_bn_apply_f32), and on the way back
 di_bn_bwd_f32 + the weight / input products.  The window attention runs in the unfused kernels of csrc/lcab_bwd.cu with
 the [P, 81] weights kept for the backward; I2P, BEVWarp sampling and the 3x3 shared convolutions have no norm and

@@ -1,4 +1,4 @@
-/* libdi_b200 -- C ABI of the B200-native (sm_100a) kernels for DeepInteraction's MMRI encoder +
+/* libdi_b200 -- C ABI of the H100-native (sm_90a) kernels for DeepInteraction's MMRI encoder +
  * MMPI decoder forward path.
  *
  * Conventions (every entry point):
@@ -30,7 +30,7 @@ extern "C" {
 
 const char* di_last_error(void);
 int di_version(void);
-int di_built_arch(void); /* 100 == sm_100a */
+int di_built_arch(void); /* 90 == sm_90a */
 
 /* Activation codes */
 #define DI_ACT_NONE 0
@@ -56,12 +56,12 @@ int di_linear_f32(const float* A0, int lda0, int K0, const float* A1, int lda1, 
 int di_conv3x3_f32(const float* x, int x_nhwc, const float* w, const float* bias, float* y, int y_nchw, int N,
                    int Cin, int H, int W, int Cout, int act, cudaStream_t stream);
 
-/* Tensor-core versions (gemm_tc.cu): error-compensated split products on tcgen05 (accumulator and the A operand
- * in tensor memory), operands staged by TMA.  Two operand precisions:
+/* Tensor-core versions (gemm_tc.cu): error-compensated split products on warpgroup MMA (wgmma; A split in registers,
+ * fp32 accumulators in registers), operands staged by TMA.  Two operand precisions:
  *   _tc_  : 3xTF32.     W_hi / W_lo  fp32 [N,K]: hi = tf32(W), lo = W - hi.             every K_s % 32 == 0
  *   _tcb_ : bf16 split. W_hi / W_mid bf16 [N,K]: hi = bf16(W), mid = bf16(W - hi).      every K_s % 64 == 0
- *           (16 mantissa bits, ~1e-5 per layer; half the tensor-pipe time and weight bytes -- the default)
- * Return -3 (unsupported) when the shape/alignment constraints are not met; the caller then falls back
+ *           (16 mantissa bits, ~1e-5 per layer; half the tensor instructions and weight bytes -- the default)
+ * Output width N % 4 == 0.  Return -3 (unsupported) when the shape/alignment constraints are not met; the caller then falls back
  * (tcb -> tc -> the FFMA entry point). */
 int di_linear_tc_f32(const float* A0, int lda0, int K0, const float* A1, int lda1, int K1, const float* A2, int lda2,
                      int K2, const float* W_hi, const float* W_lo, const float* bias, const float* res, int ldres,
@@ -74,7 +74,7 @@ int di_linear_tcb_f32(const float* A0, int lda0, int K0, const float* A1, int ld
  * (hi = bf16(x), mid = bf16(x - hi)); split_kind 1 = Q/K layout (channel pair 2j,2j+1 -> words 2j = hi, 2j+1 = mid),
  * 2 = V layout (channel group of 8 -> 4 hi words | 4 mid words); split_kind 3 = PLANAR layout for
  * di_lcab_window_tc_f32 (split_col0 % 128 == 0, N % 128 == 0): every group of 128 channels becomes 64 words of bf16
- * hi followed by 64 words of bf16 mid, i.e. two K-major bf16 planes that TMA can drop into tcgen05 operand tiles.
+ * hi followed by 64 words of bf16 mid, i.e. two bf16 planes per pixel.
  * Replaces the k/q/v projections of LocalContextAttentionBlock (models/utils/encoder_utils.py:95-131) when their
  * consumer is the window kernel. */
 int di_linear_tcb_split_f32(const float* A0, int lda0, int K0, const float* A1, int lda1, int K1, const float* A2,
@@ -110,21 +110,17 @@ int di_lcab_window_f32(const float* q, int ldq, const float* k, int ldk, const f
 int di_lcab_window_pre_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo,
                            int N, int H, int W, int C, cudaStream_t stream);
 
-/* The same op on the Blackwell tensor cores (lcab_tc.cu: tcgen05.mma with S = Q K^T and O = P V accumulated in
- * tensor memory, TMA-staged halo tiles, softmax by lane = query warps).  q, k, v: PLANAR pre-split operands
- * (split_kind 3 above) -- [N*H*W] pixels with a stride of ld* 32-bit words, 128 bf16 hi | 128 bf16 mid per pixel;
+/* The same op for PLANAR pre-split operands (split_kind 3 above; lcab.cu, bf16-split mma.sync tensor-core kernel):
+ * q, k, v -- [N*H*W] pixels with a stride of ld* 32-bit words, 128 bf16 hi | 128 bf16 mid per pixel;
  * out fp32 [N,H,W,ldo].  C must be 128 (returns -3 otherwise: use di_lcab_window_pre_f32 / di_lcab_window_f32).
  * Replaces similar_forward + softmax + weighting_forward (encoder_utils.py:132-134, localAttention.cpp:7-15,31-39). */
 int di_lcab_window_tc_f32(const void* q, int ldq, const void* k, int ldk, const void* v, int ldv, float* out, int ldo,
                           int N, int H, int W, int C, cudaStream_t stream);
-int di_lcab_window_tc_set_sm_limit(int n); /* persistent grid of the kernel above uses at most n CTAs (0 = all) */
-int di_lcab_window_tc_set_debug(int on);    /* diagnostics: clock64 pipeline trace of CTA 0 ... */
-int di_lcab_window_tc_debug_read(long long* host_buf); /* ... 6 x 256 stamps (tools/trace_window.py) */
 
 /* The five 1x1 Conv(+folded BN)+ReLU projections of LocalContextAttentionBlock (models/utils/encoder_utils.py:92-131:
  * query_project 2 layers on the target map x_t, key_project 2 layers and value_project 1 layer on the source map x_s)
- * as ONE tcgen05 launch writing q, k, v in the planar operand format of di_lcab_window_tc_f32; the first-stage
- * activations stay in tensor memory (lcab_proj.cu).  x_t / x_s [M,128] fp32 rows (x_s == x_t: self attention);
+ * as a chain of five bf16-split tensor-core GEMM launches writing q, k, v in the planar operand format of
+ * di_lcab_window_tc_f32 (lcab_proj.cu).  x_t / x_s [M,128] fp32 rows (x_s == x_t: self attention);
  * W1_hi / W1_mid [384,128] bf16 rows (q1 | k1 | v), b1 [384]; W2_hi / W2_mid [256,128] rows (q2 | k2), b2 [256];
  * q, k, v [M,128] words each (contiguous).  Results equal the unfused di_linear_tcb_split_f32 chain bit for bit. */
 int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
@@ -136,7 +132,6 @@ int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, con
 int di_lcab_forward_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
                         const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* qkv, float* out, int ldo,
                         int N, int H, int W, cudaStream_t stream);
-int di_lcab_proj_set_sm_limit(int n); /* persistent grid of the kernel above uses at most n CTAs (0 = all) */
 
 /* test/diagnostic hook: 1 = always use the FFMA window kernel, 0 = tensor-core (mma.sync 3xTF32) kernel when
  * ksize == 9 and C % 32 == 0 (default) */
@@ -402,7 +397,7 @@ int di_bev_sample_bwd_f32(const float* d_out, const float* grid_xy, float* d_bev
 int di_gather_rows_masked_f32(const float* map, const int* cnt, const int* coors, float* rows, int P, int Y, int X, int C,
                               cudaStream_t stream);
 
-/* ---- query x BEV cross attention on tcgen05 (models/utils/decoder_utils.py:101-103, 466-493; xattn_tc.cu)
+/* ---- query x BEV cross attention on the tensor cores, mma.sync bf16 split (models/utils/decoder_utils.py:101-103, 466-493; xattn_tc.cu)
  * di_attn_planes_f32: fp32 rows -> bf16 operand planes (queries, pre-scaled by head_dim^-0.5, and keys: hi | mid | lo = 192
  * words per row; values: hi | mid = 128 words); either input may be NULL.  di_xattn_tc_f32: part = float workspace of
  * B * heads * di_xattn_tc_splits(B, HW) * 18 * P; out [B*P, 128] fp32.  8 heads x 16 channels, P <= 256 (returns -3

@@ -1,4 +1,4 @@
-"""Recipe: compile the REFERENCE's own CUDA extension `localattention` for sm_100a, unmodified, from the sources
+"""Recipe: compile the REFERENCE's own CUDA extension `localattention` for sm_90a, unmodified, from the sources
 where they lie under /root/reference (projects/mmdet3d_plugin/models/utils/ops/locatt_ops/{similar.cu,weighting.cu,
 localAttention.cpp,kernels.cuh,utils.cuh,localAttention.h}) into the git-ignored oracle/_ref/.
 
@@ -8,7 +8,7 @@ under deepinteraction_b200/ or projects/ may import it.  No reference source is 
 sources are read in place, only the compiled localattention.so lands in oracle/_ref/ (which travels to the GPU box
 with the gpurun snapshot; /root/reference itself does not).
 
-Same flags as the reference's JIT recipe (locatt_ops/__init__.py:15-26) plus the explicit sm_100a -gencode (the
+Same flags as the reference's JIT recipe (locatt_ops/__init__.py:15-26) plus the explicit sm_90a -gencode (the
 reference lets torch pick the visible device's arch; there is no GPU in the build container).
 
     python oracle/build_ref.py            # -> oracle/_ref/localattention.so   (no-op if /root/reference is absent)
@@ -35,13 +35,13 @@ def build(verbose=False):
     if not os.path.isdir(REF_DIR):
         return None
     os.makedirs(OUT_DIR, exist_ok=True)
-    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '10.0a')
+    os.environ.setdefault('TORCH_CUDA_ARCH_LIST', '9.0a')
     from torch.utils import cpp_extension
     srcs = [os.path.join(REF_DIR, f) for f in ('similar.cu', 'weighting.cu', 'localAttention.cpp')]
     cpp_extension.load('localattention', sources=srcs, build_directory=OUT_DIR,
                        extra_cuda_cflags=['-DCUDA_HAS_FP16=1', '-D__CUDA_NO_HALF_OPERATORS__',
                                           '-D__CUDA_NO_HALF_CONVERSIONS__', '-D__CUDA_NO_HALF2_OPERATORS__',
-                                          '-gencode', 'arch=compute_100a,code=sm_100a'],
+                                          '-gencode', 'arch=compute_90a,code=sm_90a'],
                        is_python_module=False, verbose=verbose)
     return built_path()
 

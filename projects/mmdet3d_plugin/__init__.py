@@ -1,4 +1,4 @@
-"""Drop-in plug-in package for the DeepInteraction MMRI+MMPI forward path on B200 (libdi_b200).
+"""Drop-in plug-in package for the DeepInteraction MMRI+MMPI forward path on H100 (libdi_b200, sm_90a).
 
 Same import path and registered class names as the reference's ``projects/mmdet3d_plugin`` for the hot
 path, so ``plugin=True; plugin_dir='projects/mmdet3d_plugin/'`` in Fusion_0075_*.py resolves

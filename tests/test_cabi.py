@@ -49,7 +49,7 @@ def test_library_is_built_and_exports_header():
     for name in protos:
         assert hasattr(L, name), f'{name} declared in di_b200.h but not exported'
     assert L.di_version() >= 100
-    assert L.di_built_arch() == 100
+    assert L.di_built_arch() == 90
 
 
 def test_ctypes_signatures_match_header():

@@ -4,11 +4,12 @@ parameter gradients of the attention blocks and of the whole encoder against aut
 eval mode (folded weights) and in training mode (batch statistics; the oracle's .train() behaviour is itself pinned to the
 reference by tests/golden/{lcab,encoder}_train.pt); the I2P attention dropout with the product's mask injected into the oracle."""
 import os
-import sys
+
 
 import pytest
 import torch
 
+import locatt_cases as lc
 from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -23,28 +24,26 @@ def rows(t):           # (N, C, H, W) -> [N*H*W, C]
     return t.permute(0, 2, 3, 1).reshape(-1, t.shape[1]).contiguous()
 
 
-@pytest.mark.parametrize('N,C,H,W,ks', [(2, 128, 11, 14, 9), (1, 32, 7, 9, 9), (1, 256, 6, 5, 5)])
+@pytest.mark.parametrize('N,C,H,W,ks', lc.BACKWARD)
 def test_window_backward_kernels_match_reference_extension(N, C, H, W, ks):
-    """di_win_dot / gather / scatter (pixel-major) == the reference localattention functions (NCHW) they stand for."""
-    sys.path.insert(0, os.path.join(ROOT, 'oracle'))
-    import build_ref
-    ref = build_ref.load()
-    if ref is None:
-        pytest.skip('oracle/_ref/localattention.so not built')
+    """di_win_dot / gather / scatter (pixel-major) == the reference localattention functions (NCHW) they stand for,
+    through the extension's outputs stored in tests/golden/locatt_ref.pt (tools/make_goldens_locatt.py)."""
     from deepinteraction_b200 import ops
-    g = torch.Generator().manual_seed(7 + C)
-    a = torch.randn(N, C, H, W, generator=g).to(dev())
-    b = torch.randn(N, C, H, W, generator=g).to(dev())
-    w = torch.randn(N, H, W, ks * ks, generator=g).to(dev())
+    ref = torch.load(os.path.join(ROOT, 'tests', 'golden', lc.GOLDEN))
+    want = lambda name: ref[lc.key('backward', N, C, H, W, ks, name)]
+    a, b, w = (t.to(dev()) for t in lc.backward_inputs(N, C, H, W, ks))
     ar, br, wr = rows(a), rows(b), w.reshape(-1, ks * ks).contiguous()
     back = lambda r: r.view(N, H, W, C).permute(0, 3, 1, 2)
     tol = 3e-6
-    assert rel_err(ops.win_dot(ar, br, N, H, W, ks).view(N, H, W, -1), ref.similar_forward(a, b, ks, ks)) < tol
-    assert rel_err(back(ops.win_gather(wr, br, N, H, W, ks)), ref.weighting_forward(b, w, ks, ks)) < tol
-    assert rel_err(back(ops.win_gather(wr, br, N, H, W, ks)), ref.similar_backward(b, w, ks, ks, True)) < tol
-    assert rel_err(back(ops.win_scatter(wr, ar, N, H, W, ks)), ref.similar_backward(a, w, ks, ks, False)) < tol
-    assert rel_err(back(ops.win_scatter(wr, ar, N, H, W, ks)), ref.weighting_backward_ori(w, a, ks, ks)) < tol
-    assert rel_err(ops.win_dot(ar, br, N, H, W, ks).view(N, H, W, -1), ref.weighting_backward_weight(b, a, ks, ks)) < tol
+    dot = lc.take(ops.win_dot(ar, br, N, H, W, ks).view(N, H, W, -1))
+    gat = lc.take(back(ops.win_gather(wr, br, N, H, W, ks)))
+    sca = lc.take(back(ops.win_scatter(wr, ar, N, H, W, ks)))
+    assert rel_err(dot, want('similar_forward(a,b)')) < tol
+    assert rel_err(gat, want('weighting_forward(b,w)')) < tol
+    assert rel_err(gat, want('similar_backward(b,w,ori)')) < tol
+    assert rel_err(sca, want('similar_backward(a,w,loc)')) < tol
+    assert rel_err(sca, want('weighting_backward_ori(w,a)')) < tol
+    assert rel_err(dot, want('weighting_backward_weight(b,a)')) < tol
 
 
 def test_softmax_relu_colsum_kernels():

@@ -109,8 +109,8 @@ def test_cross_attention_matches_dense_softmax():
 
 
 @pytest.mark.parametrize('B,P,HW', [(1, 200, 32400), (2, 200, 3000), (1, 24, 1296), (3, 77, 64), (1, 256, 700)])
-def test_cross_attention_tcgen05_matches_dense_softmax(B, P, HW):
-    """di_xattn_tc_f32 (bf16 operand planes, six-term logits and three-term P V on tcgen05, online softmax, key splits) vs
+def test_cross_attention_tensor_core_matches_dense_softmax(B, P, HW):
+    """di_xattn_tc_f32 (bf16 operand planes, six-term logits and three-term P V on mma.sync, online softmax, key splits) vs
     a float64 dense softmax; the K | V rows come from the 3xTF32 GEMM like in the decoder."""
     from deepinteraction_b200 import ops, fold
     g = torch.Generator().manual_seed(P + HW)

@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_err
+from golden_sample import golden_err, shape_of
 
 pytestmark = pytest.mark.gpu
 TOL = 1e-3
@@ -140,8 +141,8 @@ def test_window_attention_presplit_operands(C, H, W):
 
 
 @pytest.mark.parametrize('N,H,W', [(2, 16, 8), (1, 40, 33), (2, 9, 50), (3, 37, 21), (1, 112, 200)])
-def test_window_attention_tcgen05_planar_operands(N, H, W):
-    """tcgen05 window kernel (lcab_tc.cu, C = 128): host-side model of the planar operand format ->
+def test_window_attention_planar_operands(N, H, W):
+    """Planar window kernel (lcab.cu, C = 128): host-side model of the planar operand format ->
     di_lcab_window_tc_f32 vs the oracle (edge tiles, several images, the base image-map shape), and
     di_linear_tcb_split_f32 kind 3 emits exactly that format."""
     import oracle.mmri as om
@@ -156,7 +157,7 @@ def test_window_attention_tcgen05_planar_operands(N, H, W):
     out = ops.lcab_window_tc(fold.split_rows(rows(q), 3), fold.split_rows(rows(k), 3), fold.split_rows(rows(v), 3),
                              N, H, W, C)
     assert rel_err(out.view(N, H, W, C).permute(0, 3, 1, 2).cpu(), ref) < TIGHT
-    # second launch on the same stream (scheduler slot re-armed, TMEM re-allocated) must reproduce the result bit for bit
+    # a second launch on the same stream must reproduce the result bit for bit
     out2 = ops.lcab_window_tc(fold.split_rows(rows(q), 3), fold.split_rows(rows(k), 3), fold.split_rows(rows(v), 3),
                               N, H, W, C)
     assert torch.equal(out, out2)
@@ -164,7 +165,8 @@ def test_window_attention_tcgen05_planar_operands(N, H, W):
 
 @pytest.mark.parametrize('M,self_attn', [(1000, True), (134400, False), (128, True), (32400, True)])
 def test_lcab_projection_chain_equals_unfused_layers(M, self_attn):
-    """di_lcab_proj_f32 (q1 / k1 kept in tensor memory) == the unfused di_linear_tcb_split_f32 chain, bit for bit."""
+    """di_lcab_proj_f32 (second stage in place over q1 / k1 in the q / k buffers) == the unfused chain through separate
+    buffers (q1 / k1 in their own tensors, then di_linear_tcb_split_f32), bit for bit."""
     from deepinteraction_b200 import ops, fold
     g = torch.Generator().manual_seed(29)
     C = 128
@@ -340,11 +342,11 @@ def test_encoder_small_matches_reference_golden(tag):
     enc = enc.to(dev()).eval()
     fr = synth.to_device(small_frame(gold['seed'], aug=gold['aug'], views=2, c_img=16, c_pts=24, bev=36, batch=2), dev())
     img, (p0, p1) = enc(fr['img_feats'], fr['pts_feats'], fr['img_metas'], fr['pts_metas'])
-    assert img.shape == gold['img'].shape and p1.shape == gold['pts'].shape
-    assert rel_err(p0.cpu(), gold['pts_conv']) < TIGHT
-    assert rel_err(p1.cpu(), gold['pts']) < TOL
-    assert rel_err(img.cpu(), gold['img']) < TOL
-    print(tag, 'rel err img %.2e pts %.2e' % (rel_err(img.cpu(), gold['img']), rel_err(p1.cpu(), gold['pts'])))
+    assert tuple(img.shape) == shape_of(gold['img']) and tuple(p1.shape) == shape_of(gold['pts'])
+    assert golden_err(p0.cpu(), gold['pts_conv']) < TIGHT
+    assert golden_err(p1.cpu(), gold['pts']) < TOL
+    assert golden_err(img.cpu(), gold['img']) < TOL
+    print(tag, 'rel err img %.2e pts %.2e' % (golden_err(img.cpu(), gold['img']), golden_err(p1.cpu(), gold['pts'])))
 
 
 @pytest.mark.parametrize('cloud,n', [('lidar', 60000), ('dense', 9000)])
@@ -396,7 +398,7 @@ def test_encoder_generates_pillars_when_not_given():
 
 
 def test_encoder_c128_matches_reference_golden():
-    """C = 128 (tcgen05 window kernel, planar operands) against a golden produced by the reference's own files."""
+    """C = 128 (planar window kernel) against a golden produced by the reference's own files."""
     from deepinteraction_b200 import mmri, synth
     from tools.make_goldens import small_frame
     import oracle.mmri as om
@@ -409,9 +411,9 @@ def test_encoder_c128_matches_reference_golden():
     enc = enc.to(dev()).eval()
     fr = synth.to_device(small_frame(gold['seed'], aug=gold['aug'], views=2, c_img=16, c_pts=24, bev=36, batch=1), dev())
     img, (p0, p1) = enc(fr['img_feats'], fr['pts_feats'], fr['img_metas'], fr['pts_metas'])
-    assert rel_err(p0.cpu(), gold['pts_conv']) < TIGHT
-    assert rel_err(p1.cpu(), gold['pts']) < TOL
-    assert rel_err(img.cpu(), gold['img']) < TOL
+    assert golden_err(p0.cpu(), gold['pts_conv']) < TIGHT
+    assert golden_err(p1.cpu(), gold['pts']) < TOL
+    assert golden_err(img.cpu(), gold['img']) < TOL
 
 
 def test_encoder_medium_c128_matches_oracle():

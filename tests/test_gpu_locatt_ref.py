@@ -1,22 +1,23 @@
-"""Kernel-level parity against the REFERENCE'S OWN CUDA extension `localattention`, compiled unmodified for sm_100a
-from /root/reference by oracle/build_ref.py into the git-ignored oracle/_ref/ (it ships with the gpurun snapshot).
+"""Kernel-level parity against the REFERENCE'S OWN CUDA extension `localattention`, through its outputs stored in
+tests/golden/locatt_ref.pt (tools/make_goldens_locatt.py ran the extension, compiled unmodified by oracle/build_ref.py,
+on the seeded inputs of tests/locatt_cases.py):
 
   (i)   the five drop-in entry points of projects/.../locatt_ops (forward + the three backward mappings, served by
         di_locatt_{cc2k,ck2c_ori,ck2c_loc}_f32) == the reference functions (localAttention.cpp:61-73), incl. non-square
         maps and kH != kW;
-  (ii)  the fused window kernels (FFMA, mma.sync 3xTF32 / bf16 split, tcgen05) == reference
+  (ii)  the fused window kernels (planar bf16 split, mma.sync 3xTF32 / bf16 split, FFMA) == reference
         similar_forward -> softmax(./sqrt(C)) -> weighting_forward (encoder_utils.py:132-134);
   (iii) the CPU oracle's window ops == the reference kernels (this pins the one op whose committed golden had to use a
         stand-in, SURVEY.md Appendix B).
 """
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import locatt_cases as lc
 from conftest import rel_err
 
 pytestmark = pytest.mark.gpu
@@ -29,12 +30,8 @@ def dev():
 
 @pytest.fixture(scope='module')
 def ref():
-    sys.path.insert(0, os.path.join(ROOT, 'oracle'))
-    import build_ref
-    mod = build_ref.load()
-    if mod is None:
-        pytest.skip('oracle/_ref/localattention.so not built (python oracle/build_ref.py needs /root/reference)')
-    return mod
+    """key -> stored output of the reference extension (all elements, or the fixed sample of locatt_cases.take)."""
+    return torch.load(os.path.join(ROOT, 'tests', 'golden', lc.GOLDEN))
 
 
 def _drop_in():
@@ -42,34 +39,19 @@ def _drop_in():
     return localattention
 
 
-@pytest.mark.parametrize('N,C,H,W,kH,kW', [(2, 16, 9, 13, 9, 9), (1, 128, 20, 17, 9, 9), (2, 8, 7, 11, 3, 5),
-                                           (1, 32, 5, 6, 5, 3)])
+@pytest.mark.parametrize('N,C,H,W,kH,kW', lc.DROP_IN)
 def test_drop_in_entry_points_equal_reference_extension(ref, N, C, H, W, kH, kW):
     ours = _drop_in()
-    g = torch.Generator().manual_seed(100 + C)
-    x_ori = torch.randn(N, C, H, W, generator=g).to(dev())
-    x_loc = torch.randn(N, C, H, W, generator=g).to(dev())
-    wgt = torch.randn(N, H, W, kH * kW, generator=g).to(dev())
-    grad_c = torch.randn(N, C, H, W, generator=g).to(dev())
+    ins = [t.to(dev()) for t in lc.drop_in_inputs(N, C, H, W, kH, kW)]
     tol = 2e-6           # both sides accumulate in fp64 and round once; the summation order differs
-    pairs = [
-        ('similar_forward', ours.similar_forward(x_ori, x_loc, kH, kW), ref.similar_forward(x_ori, x_loc, kH, kW)),
-        ('similar_backward(is_ori)', ours.similar_backward(x_loc, wgt, kH, kW, True),
-         ref.similar_backward(x_loc, wgt, kH, kW, True)),
-        ('similar_backward(is_loc)', ours.similar_backward(x_ori, wgt, kH, kW, False),
-         ref.similar_backward(x_ori, wgt, kH, kW, False)),
-        ('weighting_forward', ours.weighting_forward(x_ori, wgt, kH, kW), ref.weighting_forward(x_ori, wgt, kH, kW)),
-        ('weighting_backward_ori', ours.weighting_backward_ori(wgt, grad_c, kH, kW),
-         ref.weighting_backward_ori(wgt, grad_c, kH, kW)),
-        ('weighting_backward_weight', ours.weighting_backward_weight(x_ori, grad_c, kH, kW),
-         ref.weighting_backward_weight(x_ori, grad_c, kH, kW)),
-    ]
-    for name, a, b in pairs:
-        assert a.shape == b.shape, name
-        assert rel_err(a.cpu(), b.cpu()) < tol, name
+    for name, a in lc.drop_in_calls(ours, *ins, kH, kW).items():
+        b = ref[lc.key('drop_in', N, C, H, W, kH, kW, name)]
+        got = lc.take(a)
+        assert got.shape == b.shape, name
+        assert rel_err(got, b) < tol, name
 
 
-def test_drop_in_backward_is_the_gradient_of_the_forward(ref):
+def test_drop_in_backward_is_the_gradient_of_the_forward():
     """The backward mappings, used the way the reference's autograd Functions use them (encoder_utils.py:36-81),
     equal torch.autograd of the oracle's differentiable restatement."""
     import oracle.mmri as om
@@ -96,17 +78,14 @@ def test_drop_in_backward_is_the_gradient_of_the_forward(ref):
         assert rel_err(a.cpu().double(), b) < 2e-5, name
 
 
-@pytest.mark.parametrize('kernel', ['tcgen05', 'mma-bf16split', 'mma-3xtf32', 'ffma'])
-@pytest.mark.parametrize('N,H,W', [(2, 40, 33), (1, 17, 50)])
+@pytest.mark.parametrize('kernel', ['planar', 'mma-bf16split', 'mma-3xtf32', 'ffma'])
+@pytest.mark.parametrize('N,H,W', lc.FUSED)
 def test_fused_window_equals_reference_similar_softmax_weighting(ref, kernel, N, H, W):
     from deepinteraction_b200 import ops, fold, _lib
     C, k = 128, 9
-    g = torch.Generator().manual_seed(31 + H)
-    q, kk, v = (torch.randn(N, C, H, W, generator=g).to(dev()) for _ in range(3))
-    sim = ref.similar_forward(q, kk, k, k)
-    want = ref.weighting_forward(v, F.softmax(sim / np.sqrt(C), -1), k, k)
+    q, kk, v = (t.to(dev()) for t in lc.fused_inputs(N, H, W, C))
     rows = lambda t: t.permute(0, 2, 3, 1).reshape(-1, C).contiguous()
-    if kernel == 'tcgen05':
+    if kernel == 'planar':
         out = ops.lcab_window_tc(fold.split_rows(rows(q), 3), fold.split_rows(rows(kk), 3), fold.split_rows(rows(v), 3),
                                  N, H, W, C)
     else:
@@ -116,18 +95,16 @@ def test_fused_window_equals_reference_similar_softmax_weighting(ref, kernel, N,
         finally:
             _lib.lib().di_set_window_ffma(0)
     got = out.view(N, H, W, C).permute(0, 3, 1, 2)
-    assert rel_err(got.cpu(), want.cpu()) < 5e-5
+    assert rel_err(lc.take(got), ref[lc.key('fused', N, H, W)]) < 5e-5
 
 
 def test_cpu_oracle_window_ops_equal_reference_kernels(ref):
     import oracle.mmri as om
-    g = torch.Generator().manual_seed(5)
-    N, C, H, W, k = 2, 64, 11, 14, 9
-    q, kk, v = (torch.randn(N, C, H, W, generator=g) for _ in range(3))
+    q, kk, v, k = lc.oracle_inputs()
+    C = q.shape[1]
     sim_o = om.window_similarity(q, kk, k)
-    sim_r = ref.similar_forward(q.to(dev()), kk.to(dev()), k, k).cpu()
+    sim_r = ref[lc.key('oracle', 'sim')].view(sim_o.shape)
     assert rel_err(sim_o, sim_r) < 2e-6
     w = F.softmax(sim_r / np.sqrt(C), -1)
     out_o = om.window_weighting(v, w, k)
-    out_r = ref.weighting_forward(v.to(dev()), w.to(dev()), k, k).cpu()
-    assert rel_err(out_o, out_r) < 2e-6
+    assert rel_err(lc.take(out_o), ref[lc.key('oracle', 'out')]) < 2e-6

@@ -10,6 +10,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_err
+from golden_sample import golden_err
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -88,8 +89,8 @@ def test_plusplus_encoder_matches_reference_golden_and_oracle(tag):
     print(tag, 'vs oracle: img %.2e pts_conv %.2e pts %.2e' % errs)
     assert errs[1] < TIGHT and max(errs) < TOL
     st = gold['channel_step']
-    gerr = (rel_err(img.cpu()[:, ::st], gold['img']), rel_err(p0.cpu()[:, ::st], gold['pts_conv']),
-            rel_err(p1.cpu()[:, ::st], gold['pts']))
+    gerr = (golden_err(img.cpu()[:, ::st], gold['img']), golden_err(p0.cpu()[:, ::st], gold['pts_conv']),
+            golden_err(p1.cpu()[:, ::st], gold['pts']))
     print(tag, 'vs reference golden: img %.2e pts_conv %.2e pts %.2e' % gerr)
     assert max(gerr) < TOL
 

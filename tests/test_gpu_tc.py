@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05 (split-product, TMA-staged) dense kernels vs float64 references, and FFMA/TC agreement.
+"""GPU parity of the wgmma (split-product, TMA-staged) dense kernels vs float64 references, and FFMA/TC agreement.
 Both operand precisions (bf16 split = the default where K % 64 == 0, and 3xTF32) and both weight placements."""
 import numpy as np
 import pytest

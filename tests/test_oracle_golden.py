@@ -13,6 +13,7 @@ import oracle.mmpi as ommpi
 from deepinteraction_b200 import synth
 from tools.make_goldens import small_frame, make_decoder, state_checksum
 from conftest import rel_err
+from golden_sample import golden_err, shape_of
 
 G = os.path.join(os.path.dirname(__file__), "golden")
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -75,7 +76,7 @@ def test_encoder_small(tag):
     fr = small_frame(g['seed'], aug=g['aug'], views=2, c_img=16, c_pts=24, bev=36, batch=2)
     with torch.no_grad():
         img, (p0, p1) = m(fr['img_feats'], fr['pts_feats'], fr['img_metas'], fr['pts_metas'])
-    assert rel_err(img, g['img']) < TOL and rel_err(p0, g['pts_conv']) < TOL and rel_err(p1, g['pts']) < TOL
+    assert golden_err(img, g['img']) < TOL and golden_err(p0, g['pts_conv']) < TOL and golden_err(p1, g['pts']) < TOL
 
 
 def test_encoder_c128():
@@ -88,7 +89,7 @@ def test_encoder_c128():
     fr = small_frame(g['seed'], aug=g['aug'], views=2, c_img=16, c_pts=24, bev=36, batch=1)
     with torch.no_grad():
         img, (p0, p1) = m(fr['img_feats'], fr['pts_feats'], fr['img_metas'], fr['pts_metas'])
-    assert rel_err(img, g['img']) < TOL and rel_err(p0, g['pts_conv']) < TOL and rel_err(p1, g['pts']) < TOL
+    assert golden_err(img, g['img']) < TOL and golden_err(p0, g['pts_conv']) < TOL and golden_err(p1, g['pts']) < TOL
 
 
 def _train_step(m, inputs, cots, call):
@@ -134,18 +135,18 @@ def test_encoder_training_mode_matches_reference_golden():
         blk.I2P_block.learnedAlign.dropout = 0.0
     fr = small_frame(g['seed'], aug=True, views=2, batch=2)
     gen = torch.Generator().manual_seed(g['seed'])
-    cots = [torch.randn(o.shape, generator=gen) for o in g['outs']]
+    cots = [torch.randn(shape_of(o), generator=gen) for o in g['outs']]
     call = lambda mm, xs: (lambda r: [r[0], r[1][0], r[1][1]])(mm(xs[0], xs[1], fr['img_metas'], fr['pts_metas']))
     outs, d_in = _train_step(m, [fr['img_feats'], fr['pts_feats']], cots, call)
-    assert all(rel_err(a, b) < TOL for a, b in zip(outs, g['outs']))
-    assert all(rel_err(a, b) < 1e-4 for a, b in zip(d_in, g['d_in']))
+    assert all(golden_err(a, b) < TOL for a, b in zip(outs, g['outs']))
+    assert all(golden_err(a, b) < 1e-4 for a, b in zip(d_in, g['d_in']))
     for n, p in m.named_parameters():
         if n.endswith('out_proj.bn.bias'):          # analytically zero (cancelled by the next layer's batch mean): rounding noise
             assert float(p.grad.abs().max()) < 1e-3 and float(g['grads'][n].abs().max()) < 1e-3, n
             continue
-        assert rel_err(p.grad, g['grads'][n]) < 1e-3, n
+        assert golden_err(p.grad, g['grads'][n]) < 1e-3, n
     for n, b in m.named_buffers():
-        assert rel_err(b.float(), g['buffers'][n].float()) < 1e-5, n
+        assert golden_err(b.float(), g['buffers'][n].float()) < 1e-5, n
 
 
 @pytest.mark.parametrize('tag', ['encoder_pp_small', 'encoder_pp_nopolar'])
@@ -167,8 +168,8 @@ def test_encoder_plusplus(tag):
         img, (p0, p1) = m(list(fr['img_levels']), list(fr['pts_levels']), fr['img_metas'], fr['pts_metas'])
     st = g['channel_step']
     tol = 2e-4 if g['polar'] else 1e-5
-    assert rel_err(img[:, ::st], g['img']) < tol and rel_err(p0[:, ::st], g['pts_conv']) < 1e-6
-    assert rel_err(p1[:, ::st], g['pts']) < tol
+    assert golden_err(img[:, ::st], g['img']) < tol and golden_err(p0[:, ::st], g['pts_conv']) < 1e-6
+    assert golden_err(p1[:, ::st], g['pts']) < tol
 
 
 @pytest.mark.parametrize('tag', ['decoder_small', 'decoder_small_aug'])

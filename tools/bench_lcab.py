@@ -1,11 +1,11 @@
 #!/usr/bin/env python
 """Kernel- and module-level timing of LocalContextAttentionBlock (SURVEY.md 8(d) rows "LCAB self, image / BEV" and
-the P2I cross block) at the base shapes, for the tcgen05 window path (default) and the mma.sync path
+the P2I cross block) at the base shapes, for the planar window path with the projection chain (default), without it, and the interleaved path
 (DI_B200_WINDOW_TC=0).  Prints one JSON line per (shape, path): per-call kernel times from CUDA events, the module
 time, and the module-boundary roofline fraction (2 F bytes for self attention, 3 F for cross: each distinct input map
 read once, the output written once) against MEASURED_PEAKS.json.
 
-    python tools/bench_lcab.py [--iters 20] [--only img|bev]      (needs a B200; run through gpurun)
+    python tools/bench_lcab.py [--iters 20] [--only img|bev]      (needs an H100)
 """
 import argparse
 import json
@@ -43,9 +43,9 @@ def main():
         M = N * H * W
         x = torch.randn(M, C, device=dev)
         y = x if self_attn else torch.randn(M, C, device=dev)
-        for path in ('tcgen05+proj', 'tcgen05', 'mma.sync'):
-            ops.WINDOW_TC[0] = path != 'mma.sync'
-            ops.LCAB_PROJ[0] = path == 'tcgen05+proj'
+        for path in ('planar+proj', 'planar', 'interleaved'):
+            ops.WINDOW_TC[0] = path != 'interleaved'
+            ops.LCAB_PROJ[0] = path == 'planar+proj'
             for _ in range(3):
                 out = mmri.lcab_forward(pk, x, y, N, H, W)
             torch.cuda.synchronize()

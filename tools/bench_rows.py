@@ -1,6 +1,6 @@
 #!/usr/bin/env python
-"""Times the query-row dense layers of the decoder: di_rows_mlp_f32 vs the tcgen05 / FFMA dense kernels, each captured 20x
-in a CUDA graph so that the figure is device time per launch, not the Python launch rate (B200; run through gpurun)."""
+"""Times the query-row dense layers of the decoder: di_rows_mlp_f32 vs the wgmma / FFMA dense kernels, each captured 20x
+in a CUDA graph so that the figure is device time per launch, not the Python launch rate (needs an H100)."""
 import os
 import sys
 

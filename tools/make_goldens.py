@@ -29,6 +29,7 @@ import torch.nn as nn
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 import oracle.geometry as og          # noqa: E402
 import oracle.mmri as ommri            # noqa: E402
@@ -307,6 +308,9 @@ def main():
     def save(name, obj):
         if only and name not in only:
             return
+        if name.startswith('encoder_'):                # full-map outputs: sampled storage (tests/golden_sample.py)
+            from golden_sample import shrink
+            obj = shrink(obj)
         torch.save(obj, os.path.join(args.out, name + '.pt'))
         sz = os.path.getsize(os.path.join(args.out, name + '.pt'))
         report.append(f'{name}: {sz / 1024:.0f} KiB')
@@ -373,7 +377,7 @@ def main():
         save(tag, dict(seed=seed, aug=aug, checksum=state_checksum(om.state_dict()), img=r_img, pts_conv=r_p0,
                        pts=r_p1))
 
-    # --- G4b: encoder at the base model's hidden width (C = 128: the tcgen05 window kernel's only width) -------------
+    # --- G4b: encoder at the base model's hidden width (C = 128: the planar window kernel's only width) -------------
     if not only or 'encoder_c128' in only:
         seed = 1550
         torch.manual_seed(seed)

@@ -34,6 +34,7 @@ import torch.nn as nn
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, 'tools'))
+sys.path.insert(0, os.path.join(ROOT, 'tests'))
 
 import make_goldens as mg                 # noqa: E402
 import oracle.mmri_pp as opp               # noqa: E402
@@ -242,8 +243,9 @@ def main():
         o_img, (o_p0, o_p1) = om(list(fr['img_levels']), list(fr['pts_levels']), fr['img_metas'], fr['pts_metas'])
         print(tag, 'oracle vs reference: img %.2e pts_conv %.2e pts %.2e' % (cmp(o_img, r_img), cmp(o_p0, r_p0), cmp(o_p1, r_p1)))
         sub = 1 if polar else 4            # the second golden keeps every 4th channel (fixture size)
-        torch.save(dict(seed=seed, aug=aug, polar=polar, checksum=mg.state_checksum(om.state_dict()), channel_step=sub,
-                        img=r_img[:, ::sub].clone(), pts_conv=r_p0[:, ::sub].clone(), pts=r_p1[:, ::sub].clone()),
+        from golden_sample import shrink           # sampled storage of the larger maps (tests/golden_sample.py)
+        torch.save(shrink(dict(seed=seed, aug=aug, polar=polar, checksum=mg.state_checksum(om.state_dict()), channel_step=sub,
+                               img=r_img[:, ::sub].clone(), pts_conv=r_p0[:, ::sub].clone(), pts=r_p1[:, ::sub].clone())),
                    os.path.join(out_dir, tag + '.pt'))
         print(tag, '%.0f KiB' % (os.path.getsize(os.path.join(out_dir, tag + '.pt')) / 1024))
 

@@ -2,7 +2,7 @@
 """Per-launch timing of ONE decoder forward at the base shapes (180x180 BEV, 6 x 112x200 image maps, 200 queries):
 the launch sequence with CUDA-event times (eager), and the time of the whole decoder replayed from its CUDA graph.
 
-    python tools/profile_decoder.py [--plusplus] [--batch 1]        (needs a B200; run through gpurun)
+    python tools/profile_decoder.py [--plusplus] [--batch 1]        (needs an H100)
 """
 import argparse
 import os
