@@ -475,8 +475,9 @@ void launch_v3(dim3 grid, const CUtensorMap maps[5], const TcParams& p, cudaStre
   gemm_tc_kernel_v3<WRES, BF, ANCHW><<<grid, NTHREADS, V3_SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4], p);
 }
 
-// bf = 1: bf16-split operands (chunks of 64 k-values), 0: 3xTF32 (chunks of 32)
-int launch_tc(const CUtensorMap maps[5], const TcParams& p, int bf, cudaStream_t stream, const char* name) {
+}  // namespace
+
+int tc::sm_budget(const char* name, int* sms) {
   int devid = 0;
   cudaGetDevice(&devid);
   if (devid < 0 || devid >= MAX_DEV) {
@@ -491,7 +492,20 @@ int launch_tc(const CUtensorMap maps[5], const TcParams& p, int bf, cudaStream_t
       return DI_ERR_LAUNCH;
     }
   }
-  const int g_num_sms = ds.num_sms;
+  *sms = (g_tc_sm_limit > 0 && g_tc_sm_limit < ds.num_sms) ? g_tc_sm_limit : ds.num_sms;
+  return DI_OK;
+}
+
+namespace {
+
+// bf = 1: bf16-split operands (chunks of 64 k-values), 0: 3xTF32 (chunks of 32)
+int launch_tc(const CUtensorMap maps[5], const TcParams& p, int bf, cudaStream_t stream, const char* name) {
+  int sms = 0;
+  const int rc = sm_budget(name, &sms);
+  if (rc != DI_OK) return rc;
+  int devid = 0;
+  cudaGetDevice(&devid);
+  DevState& ds = g_dev[devid];
   if (!ds.attr_set) {
     if (cudaFuncSetAttribute(gemm_tc_kernel_v3<false, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_SMEM_BYTES) != cudaSuccess ||
         cudaFuncSetAttribute(gemm_tc_kernel_v3<true, false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, V3_SMEM_BYTES) != cudaSuccess ||
@@ -505,7 +519,6 @@ int launch_tc(const CUtensorMap maps[5], const TcParams& p, int bf, cudaStream_t
     ds.attr_set = true;
   }
   const int tiles = p.m_tiles * p.n_tiles;
-  const int sms = (g_tc_sm_limit > 0 && g_tc_sm_limit < g_num_sms) ? g_tc_sm_limit : g_num_sms;
   int nk = p.k0 + p.k1 + p.k2;
   const bool wres = !p.conv && nk <= (bf ? 2 : 4) && g_tc_wres && p.n_tiles <= 14;
   int g = tiles < sms ? tiles : sms;

@@ -4,28 +4,273 @@
 //
 //     q = relu(W_q2 relu(W_q1 x_t + b_q1) + b_q2)      k = relu(W_k2 relu(W_k1 x_s + b_k1) + b_k2)      v = relu(W_v x_s + b_v)
 //
-// written directly in the planar bf16 hi|mid operand format of the window kernel (di_lcab_window_tc_f32), as a chain of
-// five launches of the bf16-split tensor-core GEMM (gemm_tc.cu).  Each layer is the same launch the unfused chain makes,
-// so results equal the unfused path bit for bit.  The first-stage activations q1 / k1 are written into the q / k output
-// buffers and the second stage runs IN PLACE over them: with N = 128 there is one column tile, and a CTA has read all
-// A rows of a tile (every K chunk) before its epilogue writes that tile's rows, while no other CTA touches those rows.
-#include "common.cuh"
+// written directly in the planar bf16 hi|mid operand format of the window kernel (di_lcab_window_tc_f32).
+//
+// Fused kernel (default): one persistent launch.  Each CTA has one role for its lifetime -- Q (x_t -> q1 -> q),
+// K (x_s -> k1 -> k) or V (x_s -> v) -- and keeps that role's weights (bf16 hi + mid, 128 KB for Q / K, 64 KB for V)
+// resident in shared memory; the grid is split 2 : 2 : 1 in proportion to the work.  All roles walk the 64-row work
+// items in the same order at about the same rate, so the K and V (and, for self attention, Q) reads of an x tile after
+// the first are L2 hits.  The chained layer never leaves registers: the m64n128 accumulator fragment a warp holds after
+// layer 1 (bias, ReLU) is split into bf16 hi / mid and is exactly the A fragment of layer 2, so q1 / k1 are never
+// stored.  Warpgroup 0 is the TMA producer (one thread), warpgroups 1 and 2 each own whole 64-row items (alternating),
+// so one warpgroup's epilogue overlaps the other's MMA.  Every layer issues the same k-steps with the same three split
+// products in the same order as the bf16-split GEMM (gemm_tc.cu), so the results equal the five-launch chain bit for
+// bit.
+//
+// Chain (di_lcab_proj_set_mode(0)): five launches of the bf16-split GEMM, each the same launch the unfused path makes.
+// The first-stage activations q1 / k1 are written into the q / k output buffers and the second stage runs IN PLACE
+// over them: with N = 128 there is one column tile, and a CTA has read all A rows of a tile (every K chunk) before its
+// epilogue writes that tile's rows, while no other CTA touches those rows.
+#include "tc_common.cuh"
 #include "di_b200.h"
 
-extern "C" {
+namespace {
 
-// x_t / x_s [M, 128] fp32 rows (leading dimensions ld_t / ld_s; x_s == x_t for self attention).
-// W1_hi / W1_mid [384, 128] bf16 = rows (q1 | k1 | v), b1 [384]; W2_hi / W2_mid [256, 128] = rows (q2 | k2), b2 [256]
-// (BN folded; hi = bf16(W), mid = bf16(W - hi)).  q, k, v: [M, 128] 32-bit words each (contiguous), planar operands
-// of di_lcab_window_tc_f32.  C = 128 only.
-int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
-                     const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
-                     int M, cudaStream_t stream) {
-  DI_CHECK_ARG(x_t && x_s && W1_hi && W1_mid && b1 && W2_hi && W2_mid && b2 && q && k && v && M > 0, "di_lcab_proj_f32: bad argument");
-  DI_CHECK_ARG(ld_t % 4 == 0 && ld_s % 4 == 0 && ld_t >= 128 && ld_s >= 128, "di_lcab_proj_f32: leading dimensions");
-  DI_CHECK_ARG((((uintptr_t)x_t | (uintptr_t)x_s | (uintptr_t)W1_hi | (uintptr_t)W1_mid | (uintptr_t)W2_hi | (uintptr_t)W2_mid |
-                 (uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "di_lcab_proj_f32: pointers must be 16-byte aligned");
-  DI_CHECK_ARG(q != k && q != v && k != v, "di_lcab_proj_f32: q, k, v must be distinct buffers");
+using namespace tc;
+
+constexpr int PJ_ROWS = 64;                          // rows per work item (one consumer warpgroup)
+constexpr int PJ_BOX = PJ_ROWS * 32 * 4;             // 8 KB: 64 rows x 32 fp32 (one 128-byte swizzle row each)
+constexpr int PJ_STAGE = 4 * PJ_BOX;                 // 32 KB: the 64 x 128 fp32 x tile of one item
+constexpr int PJ_WBOX = 128 * 64 * 2;                // 16 KB: 128 rows x 64 bf16 of a weight
+constexpr int PJ_W_BYTES = 8 * PJ_WBOX;              // W1 hi | W1 mid | W2 hi | W2 mid of one role (2 boxes each)
+constexpr int PJ_S = 3;                              // x-tile ring stages
+constexpr int PJ_RING_BYTES = PJ_W_BYTES + PJ_S * PJ_STAGE;
+constexpr int PJ_BAR_BYTES = 64;
+constexpr int PJ_SMEM_BYTES = PJ_RING_BYTES + 1024 /*alignment*/ + PJ_BAR_BYTES;
+constexpr int PJ_THREADS = 384;
+static_assert(PJ_SMEM_BYTES <= 232448, "lcab_proj exceeds the 227 KB shared-memory limit");
+static_assert(8 * (2 * PJ_S + 1) <= PJ_BAR_BYTES, "barrier block overflow");
+
+struct ProjParams {
+  const float* b1;          // [384] = b_q1 | b_k1 | b_v
+  const float* b2;          // [256] = b_q2 | b_k2
+  uint32_t *q, *k, *v;      // planar outputs, 128 words per row
+  int M, items;             // rows, 64-row work items
+  int nq, nk, nv;           // CTAs per role (blocks [0, nq) = Q, [nq, nq + nk) = K, the rest = V)
+};
+
+// 24 wgmma (8 k-steps x 3 split products) of one 64 x 128 x 128 layer, in the order of gemm_tc_kernel_v3<.., BF = true>
+__device__ __forceinline__ void layer_mma(float (&acc)[64], const uint32_t (&ahi)[8][4], const uint32_t (&amid)[8][4],
+                                          uint32_t whi, uint32_t wmid) {
+  fence_regs(acc);
+  wgmma_fence();
+#pragma unroll
+  for (int ks = 0; ks < 8; ++ks) {
+    const uint32_t off = (ks >> 2) * PJ_WBOX + (ks & 3) * 32;
+    const uint64_t w_hi = wgmma_desc(whi + off), w_mid = wgmma_desc(wmid + off);
+    wgmma_bf16_rs(acc, amid[ks], w_hi, ks != 0);     // A_mid * W_hi
+    wgmma_bf16_rs(acc, ahi[ks], w_mid, 1);           // A_hi * W_mid
+    wgmma_bf16_rs(acc, ahi[ks], w_hi, 1);            // A_hi * W_hi
+  }
+  wgmma_commit();
+  wgmma_wait_all();
+  fence_regs(acc);
+}
+
+__device__ __forceinline__ void split_pair(float x0, float x1, uint32_t& hi, uint32_t& mid) {
+  hi = pack_bf16x2(x0, x1);
+  mid = pack_bf16x2(x0 - __uint_as_float(hi << 16), x1 - __uint_as_float(hi & 0xFFFF0000u));
+}
+
+// acc = relu(acc + bias); acc[4j + 2h + e] is (row r0 + 8h, column 8j + 2t + e) of the warp's 16 rows
+__device__ __forceinline__ void bias_relu(float (&acc)[64], const float* bias, int t) {
+#pragma unroll
+  for (int j = 0; j < 16; ++j) {
+    const float2 b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * t);
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      acc[4 * j + 2 * h] += b.x;
+      acc[4 * j + 2 * h + 1] += b.y;
+    }
+  }
+#pragma unroll
+  for (int j = 0; j < 64; ++j) acc[j] = fmaxf(acc[j], 0.f);
+}
+
+__global__ void __launch_bounds__(PJ_THREADS, 1)
+lcab_proj_kernel(const __grid_constant__ CUtensorMap mapXt, const __grid_constant__ CUtensorMap mapXs,
+                 const __grid_constant__ CUtensorMap mapW1h, const __grid_constant__ CUtensorMap mapW1m,
+                 const __grid_constant__ CUtensorMap mapW2h, const __grid_constant__ CUtensorMap mapW2m,
+                 const ProjParams p) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint8_t* base_ptr = smem_raw + (base - smem_u32(smem_raw));
+  const uint32_t bars = base + PJ_RING_BYTES;
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (PJ_S + s); };
+  const uint32_t w_full = bars + 8u * (2 * PJ_S);
+
+  const int bid = blockIdx.x;
+  const int role = bid < p.nq ? 0 : (bid < p.nq + p.nk ? 1 : 2);        // 0 = Q, 1 = K, 2 = V
+  const int first = role == 0 ? bid : (role == 1 ? bid - p.nq : bid - p.nq - p.nk);
+  const int stride = role == 0 ? p.nq : (role == 1 ? p.nk : p.nv);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < PJ_S; ++s) {
+      mbar_init(full(s), 1);
+      mbar_init(empty(s), 4);                        // the four warps of the consuming warpgroup
+    }
+    mbar_init(w_full, 1);
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  if (warp < 4) {
+    // ---------------- TMA producer (one thread) ----------------
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 40;");
+    if (threadIdx.x == 0) {
+      const int wrow = role * 128;                   // this role's 128 output channels in W1 / W2
+      mbar_expect_tx(w_full, (role == 2 ? 4 : 8) * PJ_WBOX);
+      for (int kc = 0; kc < 2; ++kc) {
+        tma_load_2d(base + kc * PJ_WBOX, &mapW1h, w_full, kc * 64, wrow);
+        tma_load_2d(base + (2 + kc) * PJ_WBOX, &mapW1m, w_full, kc * 64, wrow);
+        if (role != 2) {
+          tma_load_2d(base + (4 + kc) * PJ_WBOX, &mapW2h, w_full, kc * 64, wrow);
+          tma_load_2d(base + (6 + kc) * PJ_WBOX, &mapW2m, w_full, kc * 64, wrow);
+        }
+      }
+      const CUtensorMap* mx = role == 0 ? &mapXt : &mapXs;
+      int n = 0;
+      for (int item = first; item < p.items; item += stride, ++n) {
+        const int s = n % PJ_S;
+        if (n >= PJ_S) mbar_wait(empty(s), ((n / PJ_S) - 1) & 1);
+        const uint32_t st = base + PJ_W_BYTES + s * PJ_STAGE;
+        mbar_expect_tx(full(s), PJ_STAGE);
+        for (int b = 0; b < 4; ++b) tma_load_2d(st + b * PJ_BOX, mx, full(s), 32 * b, item * PJ_ROWS);
+        const int ahead = item + PJ_S * stride;      // the item this stage is loaded with next: L2 prefetch
+        if (ahead < p.items)
+          for (int b = 0; b < 4; ++b) tma_prefetch_2d(mx, 32 * b, ahead * PJ_ROWS);
+      }
+    }
+  } else {
+    // ---------------- consumers: warpgroup 1 takes the CTA's even items, warpgroup 2 the odd ones ----------------
+    asm volatile("setmaxnreg.inc.sync.aligned.u32 232;");
+    const int wg = (warp >> 2) - 1, wl = warp & 3;
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = wl * 16 + g, r1 = r0 + 8;         // item rows of this thread's fragments
+    const uint32_t w1h = base, w1m = base + 2 * PJ_WBOX, w2h = base + 4 * PJ_WBOX, w2m = base + 6 * PJ_WBOX;
+    const float* b1 = p.b1 + role * 128;
+    const float* b2 = p.b2 + role * 128;
+    uint32_t* out = role == 0 ? p.q : (role == 1 ? p.k : p.v);
+    mbar_wait(w_full, 0);
+    float acc[64];
+    uint32_t ahi[8][4], amid[8][4];
+    int n = wg;
+    for (int item = first + wg * stride; item < p.items; item += 2 * stride, n += 2) {
+      const int s = n % PJ_S;
+      mbar_wait(full(s), (n / PJ_S) & 1);
+      // landed x tile -> bf16 hi / mid A fragments of all 8 k-steps; the stage is free as soon as they are in registers
+      const float* xt = reinterpret_cast<const float*>(base_ptr + PJ_W_BYTES + s * PJ_STAGE);
+#pragma unroll
+      for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          const int row = (e & 1) ? r1 : r0, c = 16 * ks + 2 * t + 8 * (e >> 1);
+          const int b = c >> 5, kk = c & 31;
+          const float2 x = *reinterpret_cast<const float2*>(xt + b * (PJ_BOX / 4) + row * 32 +
+                                                            (((kk >> 2) ^ (row & 7)) << 2) + (kk & 3));
+          split_pair(x.x, x.y, ahi[ks][e], amid[ks][e]);
+        }
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(s));
+      layer_mma(acc, ahi, amid, w1h, w1m);
+      bias_relu(acc, b1, t);
+      if (role != 2) {
+        // q1 / k1 fragment -> A fragment of layer 2: k-step ks = columns 16 ks .. 16 ks + 15 = accumulator pairs j = 2 ks, 2 ks + 1
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks)
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const int a = 4 * (2 * ks + (e >> 1)) + 2 * (e & 1);
+            split_pair(acc[a], acc[a + 1], ahi[ks][e], amid[ks][e]);
+          }
+        layer_mma(acc, ahi, amid, w2h, w2m);
+        bias_relu(acc, b2, t);
+      }
+      // planar epilogue: per row 64 words of bf16 hi pairs, then 64 words of bf16 mid pairs
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int row = item * PJ_ROWS + (h ? r1 : r0);
+        if (row >= p.M) continue;
+        uint32_t* orow = out + (size_t)row * 128;
+#pragma unroll
+        for (int j = 0; j < 16; ++j) {
+          uint32_t hi, mid;
+          split_pair(acc[4 * j + 2 * h], acc[4 * j + 2 * h + 1], hi, mid);
+          orow[4 * j + t] = hi;
+          orow[64 + 4 * j + t] = mid;
+        }
+      }
+    }
+  }
+}
+
+bool make_map(CUtensorMap* m, CUtensorMapDataType dt, const void* ptr, long long rows, long long cols, long long ld_bytes,
+              int box_cols, int box_rows) {
+  EncodeTiledFn enc = get_encode();
+  if (!enc) return false;
+  cuuint64_t dims[2] = {(cuuint64_t)cols, (cuuint64_t)rows};
+  cuuint64_t strides[1] = {(cuuint64_t)ld_bytes};
+  cuuint32_t box[2] = {(cuuint32_t)box_cols, (cuuint32_t)box_rows};
+  cuuint32_t estr[2] = {1, 1};
+  return enc(m, dt, 2, const_cast<void*>(ptr), dims, strides, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
+             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
+}
+
+constexpr int MAX_DEV = 64;
+bool g_attr_set[MAX_DEV];
+int g_fused = 1;
+
+int proj_fused(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
+               const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
+               int M, cudaStream_t stream) {
+  const char* name = "di_lcab_proj_f32";
+  int sms = 0;
+  int rc = sm_budget(name, &sms);
+  if (rc != DI_OK) return rc;
+  int devid = 0;
+  cudaGetDevice(&devid);
+  if (!g_attr_set[devid]) {
+    if (cudaFuncSetAttribute(lcab_proj_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, PJ_SMEM_BYTES) != cudaSuccess) {
+      di_set_error("%s: cannot reserve %d bytes of shared memory", name, PJ_SMEM_BYTES);
+      return DI_ERR_LAUNCH;
+    }
+    g_attr_set[devid] = true;
+  }
+  CUtensorMap maps[6];
+  const auto bf16 = CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, f32 = CU_TENSOR_MAP_DATA_TYPE_FLOAT32;
+  if (!(make_map(&maps[0], f32, x_t, M, 128, 4ll * ld_t, 32, PJ_ROWS) && make_map(&maps[1], f32, x_s, M, 128, 4ll * ld_s, 32, PJ_ROWS) &&
+        make_map(&maps[2], bf16, W1_hi, 384, 128, 256, 64, 128) && make_map(&maps[3], bf16, W1_mid, 384, 128, 256, 64, 128) &&
+        make_map(&maps[4], bf16, W2_hi, 256, 128, 256, 64, 128) && make_map(&maps[5], bf16, W2_mid, 256, 128, 256, 64, 128))) {
+    di_set_error("%s: cuTensorMapEncodeTiled failed", name);
+    return DI_ERR_LAUNCH;
+  }
+  ProjParams p{};
+  p.b1 = b1;
+  p.b2 = b2;
+  p.q = reinterpret_cast<uint32_t*>(q);
+  p.k = reinterpret_cast<uint32_t*>(k);
+  p.v = reinterpret_cast<uint32_t*>(v);
+  p.M = M;
+  p.items = di_cdiv(M, PJ_ROWS);
+  // Q : K : V = 2 : 2 : 1 (V is one layer, Q and K two), at least one CTA per role, none without an item
+  const int G = sms > 3 ? sms : 3;
+  const int nv = G / 5 > 1 ? G / 5 : 1;
+  const int nq = (G - nv + 1) / 2;
+  const int nk = G - nv - nq;
+  p.nq = nq < p.items ? nq : p.items;
+  p.nk = nk < p.items ? nk : p.items;
+  p.nv = nv < p.items ? nv : p.items;
+  lcab_proj_kernel<<<p.nq + p.nk + p.nv, PJ_THREADS, PJ_SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], maps[3], maps[4],
+                                                                                maps[5], p);
+  DI_CHECK_LAUNCH(name);
+  return DI_OK;
+}
+
+int proj_chain(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
+               const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
+               int M, cudaStream_t stream) {
   constexpr size_t WB = 128 * 128 * 2;               // bytes of one 128 x 128 bf16 weight block
   auto w = [&](const void* p, int blk) { return static_cast<const void*>(static_cast<const char*>(p) + blk * WB); };
   struct Layer {
@@ -46,7 +291,33 @@ int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, con
   return DI_OK;
 }
 
-// LocalContextAttentionBlock.forward (models/utils/encoder_utils.py:119-135) for C = 128 as ONE call: the projection chain
+}  // namespace
+
+extern "C" {
+
+// 1 (default): the fused kernel; 0: the five-launch chain (A/B runs and tests)
+int di_lcab_proj_set_mode(int mode) {
+  DI_CHECK_ARG(mode == 0 || mode == 1, "di_lcab_proj_set_mode: mode must be 0 or 1");
+  g_fused = mode;
+  return DI_OK;
+}
+
+// x_t / x_s [M, 128] fp32 rows (leading dimensions ld_t / ld_s; x_s == x_t for self attention).
+// W1_hi / W1_mid [384, 128] bf16 = rows (q1 | k1 | v), b1 [384]; W2_hi / W2_mid [256, 128] = rows (q2 | k2), b2 [256]
+// (BN folded; hi = bf16(W), mid = bf16(W - hi)).  q, k, v: [M, 128] 32-bit words each (contiguous), planar operands
+// of di_lcab_window_tc_f32.  C = 128 only.
+int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
+                     const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
+                     int M, cudaStream_t stream) {
+  DI_CHECK_ARG(x_t && x_s && W1_hi && W1_mid && b1 && W2_hi && W2_mid && b2 && q && k && v && M > 0, "di_lcab_proj_f32: bad argument");
+  DI_CHECK_ARG(ld_t % 4 == 0 && ld_s % 4 == 0 && ld_t >= 128 && ld_s >= 128, "di_lcab_proj_f32: leading dimensions");
+  DI_CHECK_ARG((((uintptr_t)x_t | (uintptr_t)x_s | (uintptr_t)W1_hi | (uintptr_t)W1_mid | (uintptr_t)W2_hi | (uintptr_t)W2_mid |
+                 (uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "di_lcab_proj_f32: pointers must be 16-byte aligned");
+  DI_CHECK_ARG(q != k && q != v && k != v, "di_lcab_proj_f32: q, k, v must be distinct buffers");
+  return (g_fused ? proj_fused : proj_chain)(x_t, ld_t, x_s, ld_s, W1_hi, W1_mid, b1, W2_hi, W2_mid, b2, q, k, v, M, stream);
+}
+
+// LocalContextAttentionBlock.forward (models/utils/encoder_utils.py:119-135) for C = 128 as ONE call: the projections
 // (di_lcab_proj_f32) followed by the window kernel (di_lcab_window_tc_f32) on `stream`.  x_t / x_s [N*H*W, 128]
 // fp32 pixel-major rows (x_s == x_t: self attention), folded weights as for di_lcab_proj_f32, qkv: workspace of
 // 3 * N*H*W * 128 32-bit words (16-byte aligned), out [N*H*W, ldo] fp32.  This is the entry SURVEY.md 8(b) calls

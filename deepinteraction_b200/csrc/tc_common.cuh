@@ -117,4 +117,8 @@ inline EncodeTiledFn get_encode() {
   return fn;
 }
 
+// CTAs a persistent tensor-core grid may use on the current device: its SM count, capped by di_tc_set_sm_limit
+// (gemm_tc.cu).  Returns DI_OK or an error status with the message set.
+int sm_budget(const char* name, int* sms);
+
 }  // namespace tc

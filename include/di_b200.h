@@ -119,13 +119,17 @@ int di_lcab_window_tc_f32(const void* q, int ldq, const void* k, int ldk, const 
 
 /* The five 1x1 Conv(+folded BN)+ReLU projections of LocalContextAttentionBlock (models/utils/encoder_utils.py:92-131:
  * query_project 2 layers on the target map x_t, key_project 2 layers and value_project 1 layer on the source map x_s)
- * as a chain of five bf16-split tensor-core GEMM launches writing q, k, v in the planar operand format of
- * di_lcab_window_tc_f32 (lcab_proj.cu).  x_t / x_s [M,128] fp32 rows (x_s == x_t: self attention);
- * W1_hi / W1_mid [384,128] bf16 rows (q1 | k1 | v), b1 [384]; W2_hi / W2_mid [256,128] rows (q2 | k2), b2 [256];
- * q, k, v [M,128] words each (contiguous).  Results equal the unfused di_linear_tcb_split_f32 chain bit for bit. */
+ * writing q, k, v in the planar operand format of di_lcab_window_tc_f32 (lcab_proj.cu).  By default ONE persistent
+ * wgmma launch: each CTA has a Q, K or V role with that role's weights resident in shared memory, and the first-stage
+ * activations q1 / k1 stay in registers (each x tile read from HBM once, q, k, v written once).  x_t / x_s [M,128] fp32
+ * rows (x_s == x_t: self attention; ld >= 128, ld % 4 == 0); W1_hi / W1_mid [384,128] bf16 rows (q1 | k1 | v), b1 [384];
+ * W2_hi / W2_mid [256,128] rows (q2 | k2), b2 [256]; q, k, v [M,128] words each (contiguous, distinct); 16-byte aligned
+ * pointers.  Results equal the unfused di_linear_tcb_split_f32 chain bit for bit. */
 int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
                      const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
                      int M, cudaStream_t stream);
+/* 1 = the fused kernel (default), 0 = five separate bf16-split GEMM launches (process-wide; A/B runs and tests) */
+int di_lcab_proj_set_mode(int mode);
 
 /* LocalContextAttentionBlock.forward for C = 128 as one call = di_lcab_proj_f32 + di_lcab_window_tc_f32 on `stream`
  * (models/utils/encoder_utils.py:119-135; SURVEY.md 8(b) `di_lcab_forward`).  qkv: workspace of 3 * N*H*W * 128 words. */
