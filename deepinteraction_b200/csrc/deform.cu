@@ -380,8 +380,9 @@ int di_axpy_f32(const float* a, const float* b, const float* scale, float* out, 
 // map[coors[p]] += rows[p, :] where cnt[p] > 0 (n_dev as in di_scatter_rows_f32)
 int di_scatter_rows_add_f32(const float* rows, const int* cnt, const int* coors, float* map, int P, int Y, int X, int C,
                             const int* n_dev, cudaStream_t stream) {
-  DI_CHECK_ARG(map && coors && rows && cnt && P >= 0 && C % 4 == 0, "di_scatter_rows_add_f32: bad argument");
-  if (P == 0) return DI_OK;
+  DI_CHECK_ARG(P >= 0 && C % 4 == 0, "di_scatter_rows_add_f32: bad argument");
+  if (P == 0) return DI_OK;                     // empty tensors may have null data pointers
+  DI_CHECK_ARG(map && coors && rows && cnt, "di_scatter_rows_add_f32: null pointer");
   scatter_rows_add_kernel<<<di_cdiv(P, 8), 256, 0, stream>>>(rows, cnt, coors, map, P, Y, X, C, n_dev);
   DI_CHECK_LAUNCH("di_scatter_rows_add_f32");
   return DI_OK;

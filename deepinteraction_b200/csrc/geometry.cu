@@ -765,8 +765,9 @@ extern "C" {
 // configurations and buffer addresses independent of the per-frame pillar / point counts (CUDA-graph replay).
 int di_gather_rows_f32(const float* map, const int* coors, float* rows, int P, int Y, int X, int C, const int* n_dev,
                        cudaStream_t stream) {
-  DI_CHECK_ARG(map && coors && rows && P >= 0 && C % 4 == 0, "di_gather_rows_f32: bad argument");
-  if (P == 0) return DI_OK;
+  DI_CHECK_ARG(P >= 0 && C % 4 == 0, "di_gather_rows_f32: bad argument");
+  if (P == 0) return DI_OK;                     // empty tensors may have null data pointers
+  DI_CHECK_ARG(map && coors && rows, "di_gather_rows_f32: null pointer");
   gather_rows_kernel<<<di_cdiv(P, 8), 256, 0, stream>>>(map, coors, rows, P, Y, X, C, n_dev);
   DI_CHECK_LAUNCH("di_gather_rows_f32");
   return DI_OK;
@@ -774,8 +775,9 @@ int di_gather_rows_f32(const float* map, const int* coors, float* rows, int P, i
 
 int di_scatter_rows_f32(const float* rows, const int* cnt, const int* coors, float* map, int P, int Y, int X, int C,
                         const int* n_dev, cudaStream_t stream) {
-  DI_CHECK_ARG(map && coors && rows && cnt && P >= 0 && C % 4 == 0, "di_scatter_rows_f32: bad argument");
+  DI_CHECK_ARG(P >= 0 && C % 4 == 0, "di_scatter_rows_f32: bad argument");
   if (P == 0) return DI_OK;
+  DI_CHECK_ARG(map && coors && rows && cnt, "di_scatter_rows_f32: null pointer");
   scatter_rows_kernel<<<di_cdiv(P, 8), 256, 0, stream>>>(rows, cnt, coors, map, P, Y, X, C, n_dev);
   DI_CHECK_LAUNCH("di_scatter_rows_f32");
   return DI_OK;
@@ -871,8 +873,9 @@ int di_i2p_dropout_mask_f32(float* mask, int P, int S, float pdrop, unsigned int
 // rows[p] = cnt[p] > 0 ? map[coors[p]] : 0 : the gradient that reaches the attention output of pillar p
 int di_gather_rows_masked_f32(const float* map, const int* cnt, const int* coors, float* rows, int P, int Y, int X, int C,
                               cudaStream_t stream) {
-  DI_CHECK_ARG(map && cnt && coors && rows && P >= 0 && C % 4 == 0, "di_gather_rows_masked_f32: bad argument");
+  DI_CHECK_ARG(P >= 0 && C % 4 == 0, "di_gather_rows_masked_f32: bad argument");
   if (P == 0) return DI_OK;
+  DI_CHECK_ARG(map && cnt && coors && rows, "di_gather_rows_masked_f32: null pointer");
   gather_rows_masked_kernel<<<di_cdiv(P, 8), 256, 0, stream>>>(map, cnt, coors, rows, P, Y, X, C);
   DI_CHECK_LAUNCH("di_gather_rows_masked_f32");
   return DI_OK;

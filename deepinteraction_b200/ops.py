@@ -404,13 +404,13 @@ def i2p_attend(qk, pillars, npts, coors, proj, img_nhwc, V, in_hw, n_dev=None, d
     _, T, pdim = pillars.shape
     BV, h, w, Ci = img_nhwc.shape
     assert Ci == C and pillars.is_contiguous() and img_nhwc.is_contiguous()
-    s = torch.empty(P, C, device=qk.device, dtype=torch.float32)
+    drop = dropout is not None and dropout[0] > 0
+    s = torch.empty(P, C + 4 if drop else C, device=qk.device, dtype=torch.float32)
     cnt = torch.empty(P, device=qk.device, dtype=torch.int32)
     if n_dev is not None:
         s.zero_()                       # rows beyond the live count feed a dense layer: keep them finite
     nb = 4 * (2 * P * C + pillars.numel() + img_nhwc.numel())
-    if dropout is not None and dropout[0] > 0:
-        s = torch.empty(P, C + 4, device=qk.device, dtype=torch.float32)
+    if drop:
         _call('di_i2p_attend_dropout_f32', _ptr(qk), _ptr(pillars), _ptr(npts), _ptr(coors), _ptr(proj), _ptr(img_nhwc), _ptr(s),
               _ptr(cnt), P, T, pdim, V, h, w, C, in_hw[0], in_hw[1], _ptr(n_dev), float(dropout[0]), int(dropout[1]) & 0xFFFFFFFF,
               _stream(), nbytes=nb)
