@@ -27,6 +27,9 @@ SIGNATURES = {
     'di_attn_planes_f32': [_p, _i, _p, _i, _p, _i, _p, _p, _ll, _p],
     'di_xattn_tc_splits': [_i, _i],
     'di_xattn_tc_f32': [_p, _p, _p, _p, _p, _i, _i, _i, _i, _p],
+    'di_xattn_tc_lse_f32': [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p],
+    'di_xattn_bwd_workspace': [_i, _i, _i],
+    'di_xattn_bwd_f32': [_p, _p, _p, _p, _p, _i, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     'di_conv3x3_tc_f32': [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_conv3x3_tcb_f32': [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_conv3x3_tc_nchw_f32': [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
@@ -69,6 +72,7 @@ SIGNATURES = {
     'di_topk_f32': [_p, _p, _i, _i, _i, _p, _i, _p],
     'di_query_init_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_mha_small_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _p],
+    'di_mha_small_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _i, _i, _i, _i, _p],
     'di_cross_attn_f32': [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_rows_finish_f32': [_p, _i, _ll, _i, _p, _p, _i, _p, _p, _p, _i, _p, _i, _i, _i, _f, _p],
     'di_rows_mlp_f32': [_p, _i, _i, _p, _i, _i, _p, _p, _i, _i, _p, _p, _i, _p, _i, _p, _p, _f, _i, _p, _p, _i, _i, _p],
@@ -86,6 +90,7 @@ SIGNATURES = {
     'di_win_softmax_bwd_f32': [_p, _p, _p, _ll, _i, _f, _p],
     'di_relu_bwd_f32': [_p, _p, _p, _ll, _p],
     'di_col_sum_f32': [_p, _i, _ll, _i, _p, _p, _p],
+    'di_ln_bwd_f32': [_p, _i, _p, _i, _p, _p, _i, _p, _p, _p, _i, _i, _f, _p],
     'di_shift_map_f32': [_p, _p, _i, _i, _i, _i, _i, _i, _p],
     # bn_train.cu
     'di_bn_stats_f32': [_p, _ll, _i, _p, _p, _p, _p, _p, _f, _p],

@@ -1,4 +1,4 @@
-"""Backward of LocalContextAttentionBlock on libdi_b200 (SURVEY.md 8(b) `di_lcab_backward`, the training side of the
+"""Backward of LocalContextAttentionBlock, of the encoder and of the decoder's query x BEV transformer layer on libdi_b200 (SURVEY.md 8(b) `di_lcab_backward`, the training side of the
 hot module; forward: mmri.lcab_forward / di_lcab_forward_f32).
 
 Reference: models/utils/encoder_utils.py:36-81 (autograd Functions around the window ops: similar_backward x 2,
@@ -273,3 +273,114 @@ class LCABFunction(torch.autograd.Function):
         target, source = ctx.saved_tensors
         r = lcab_backward(ctx.pk, target, target if ctx.same else source, *ctx.dims, grad_out)
         return None, r['d_target'], r['d_source'], None, None, None
+
+
+# ---- decoder: TransformerDecoderLayer (query x BEV) ---------------------------------------------------------------------
+def _dec_bw_pack(dec, pk):
+    """Transposed weights of the layer's dX products and the constants of fold.decoder_layer_unfold, built once per pack."""
+    if '_bw' in pk:
+        return pk['_bw']
+    layer = dec.decoder[0]
+    dev = pk['bce'].device
+    C = dec.hidden_channel
+    T = lambda w: fold.Weight(fold._d(w).reshape(w.shape[0], -1).t().contiguous(), dev)
+    s = float(C // dec.num_heads) ** -0.5
+    w_in = fold._d(layer.self_attn.in_proj_weight).clone()
+    w_in[:C] *= s
+    w_x = fold._d(layer.multihead_attn.in_proj_weight).clone()
+    w_x[:C] *= s
+    Td = lambda w: fold.Weight(w.t().contiguous(), dev)
+    pk['_bw'] = dict(ffn2=T(layer.linear2.weight), ffn1=T(layer.linear1.weight), cross_out=T(layer.multihead_attn.out_proj.weight),
+                     self_out=T(layer.self_attn.out_proj.weight), cross_q=Td(w_x[:C]), kv=Td(w_x[C:]), self_in=Td(w_in),
+                     spe2=T(layer.self_posembed.position_embedding_head[3].weight),
+                     cpe2=T(layer.cross_posembed.position_embedding_head[3].weight),
+                     unfold=fold.decoder_layer_unfold_consts(layer, dec.num_heads, dev), one=torch.ones(1, device=dev))
+    return pk['_bw']
+
+
+def decoder_layer_backward(dec, query, query_pos, bev, grad_out):
+    """Backward of the decoder's TransformerDecoderLayer (reference models/utils/decoder_utils.py:35-113, 116-495; the call
+    self.decoder[0](query_feat, lidar_feat_flatten, query_pos, bev_pos) of deepinteraction_decoder.py), shared by the base
+    and the ++ decoder, with BatchNorm in eval mode (the folded weights of the forward) and dropout off.
+    dec: DeepInteractionDecoder / DeepInteractionPlusPlusDecoder on the GPU; query [B*P, C] and query_pos [B*P, 2]: the rows
+    the forward feeds the layer; bev [B, Y, X, C]: pts_conv (pixel-major); grad_out [B*P, C].
+    -> dict(d_query [B*P, C], d_bev [B, Y, X, C] (through K and V), grads = {name: tensor} for the 30 parameters of
+    dec.decoder[0], keyed and shaped as in its state_dict).  query_pos gets no gradient (a gather of the constant bev_pos).
+    The layer is re-run eagerly with its intermediates kept; everything stays on the device, without host synchronisation
+    after the first call of a pack."""
+    with _precise():
+        return _decoder_layer_backward(dec, query, query_pos, bev, grad_out)
+
+
+def _decoder_layer_backward(dec, query, query_pos, bev, grad_out):
+    pk = dec.pack()
+    C, H = dec.hidden_channel, dec.num_heads
+    B, Y, X, _ = bev.shape
+    HW, M = Y * X, query.shape[0]
+    P = M // B
+    if H != 8 or C != 128 or P > 256 or P * B != M:
+        raise NotImplementedError('decoder_layer_backward: the cross-attention gradient kernel takes 8 heads x 16 channels and '
+                                  f'P <= 256 queries per sample (got heads={H}, C={C}, rows={M}, B={B})')
+    bw = _dec_bw_pack(dec, pk)
+    query, query_pos, bev = query.contiguous(), query_pos.contiguous(), bev.contiguous()
+    sv = {}
+    dec._layer(pk, query, query_pos, bev, B, P, saved=sv)
+    add = lambda a, b: ops.axpy(a.contiguous(), b.contiguous(), bw['one'])
+    R, F = {}, {}
+    # norm3, FFN
+    dz3, R['norm3.weight'], R['norm3.bias'] = ops.ln_bwd(grad_out.contiguous(), sv['z3'], pk['norm3'][0])
+    R['linear2.weight'], R['linear2.bias'] = _wgrad(dz3, sv['f']), ops.col_sum(dz3)
+    df = ops.relu_bwd(ops.linear([dz3], bw['ffn2']), sv['f'])
+    R['linear1.weight'], R['linear1.bias'] = _wgrad(df, sv['q2']), ops.col_sum(df)
+    dq2 = ops.linear([df], bw['ffn1'], res=dz3)
+    # norm2, query x BEV cross attention
+    dz2, R['norm2.weight'], R['norm2.bias'] = ops.ln_bwd(dq2, sv['z2'], pk['norm2'][0])
+    R['multihead_attn.out_proj.weight'], R['multihead_attn.out_proj.bias'] = _wgrad(dz2, sv['a2']), ops.col_sum(dz2)
+    da2 = ops.linear([dz2], bw['cross_out'])
+    dqc, dkv = ops.xattn_bwd(sv['planes'], sv['a2'], sv['lse'], da2, B, P, HW, H)
+    F['cross_q'] = (_wgrad(dqc, torch.cat([sv['q1'], sv['qpe']], 1)), ops.col_sum(dqc))
+    F['cross_kv'] = (_wgrad(dkv, sv['kk']), ops.col_sum(dkv))
+    tq = ops.linear([dqc], bw['cross_q'])               # the [Wq | Wq] pack: the same gradient for q1 and qpe
+    d_bev = ops.linear([dkv], bw['kv'])                 # d kk [B*HW, C] = d bev
+    # constant key positional embedding: d kpe = sum over the batch of d kk, back through its MLP over the grid positions
+    dkpe = d_bev[:HW]
+    for b in range(1, B):
+        dkpe = add(dkpe, d_bev[b * HW:(b + 1) * HW])
+    cpe = pk['cross_pe']
+    dh = ops.relu_bwd(ops.linear([dkpe.contiguous()], bw['cpe2']), cpe['hidden'])
+    F['cross_posembed'] = (_wgrad(dh, cpe['pos']), ops.col_sum(dh), _wgrad(dkpe.contiguous(), cpe['hidden']), ops.col_sum(dkpe))
+    # norm1, self attention over the queries
+    dz1, R['norm1.weight'], R['norm1.bias'] = ops.ln_bwd(add(dz2, tq), sv['z1'], pk['norm1'][0])
+    R['self_attn.out_proj.weight'], R['self_attn.out_proj.bias'] = _wgrad(dz1, sv['a1']), ops.col_sum(dz1)
+    da1 = ops.linear([dz1], bw['self_out'])
+    qkv = sv['qkv']
+    dqkv = ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da1, B, P, H)
+    F['self_in'] = (_wgrad(dqkv, torch.cat([query, sv['qpe']], 1)), ops.col_sum(dqkv))
+    ts = ops.linear([dqkv], bw['self_in'])              # the [W | W] pack: the same gradient for query and qpe
+    d_query = add(dz1, ts)
+    dqpe = add(tq, ts)
+    # self positional MLP
+    dhs = ops.relu_bwd(ops.linear([dqpe], bw['spe2']), sv['hs'])
+    F['self_posembed'] = (_wgrad(dhs, query_pos), ops.col_sum(dhs), _wgrad(dqpe, sv['hs']), ops.col_sum(dqpe))
+    R.update(fold.decoder_layer_unfold(bw['unfold'], F))
+    return dict(d_query=d_query, d_bev=d_bev.view(B, Y, X, C), grads=R)
+
+
+class DecoderLayerFunction(torch.autograd.Function):
+    """autograd wrapper: out [B*P, C] = the decoder's TransformerDecoderLayer (the forward schedule's kernels, bit for bit);
+    backward -> (d_query, d_bev) through decoder_layer_backward.  Parameter gradients are returned by decoder_layer_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, query, query_pos, bev):
+        ctx.dec = dec
+        ctx.save_for_backward(query, query_pos, bev)
+        with _precise():
+            pk = dec.pack()
+            B = bev.shape[0]
+            return dec._layer(pk, query.contiguous(), query_pos.contiguous(), bev.contiguous(), B, query.shape[0] // B)
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        query, query_pos, bev = ctx.saved_tensors
+        r = decoder_layer_backward(ctx.dec, query, query_pos, bev, grad_out)
+        return None, r['d_query'], None, r['d_bev']

@@ -295,6 +295,124 @@ mha_small_kernel(const float* __restrict__ q, int ldq, const float* __restrict__
   }
 }
 
+// Backward of mha_small_kernel without group masks (the transformer layer's self-attention, decoder_utils.py:95-99).
+// Pass 1, one warp per (query i, head): recompute A_i = softmax(q_i K^T), dA_ij = dO_i . v_j, D_i = sum_j A_ij dA_ij,
+// dS_ij = A_ij (dA_ij - D_i), dq_i = sum_j dS_ij k_j; A and dS are stored key-major ([b, head, j, i]) for pass 2.
+// Pass 2, one warp per (key j, head): dk_j = sum_i dS_ij q_i, dv_j = sum_i A_ij dO_i.  Fixed summation orders (lanes
+// over a strided index range, then the warp butterfly): deterministic, no atomics.
+template <int D>
+__global__ void __launch_bounds__(256)
+mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk, const float* __restrict__ v,
+                       int ldv, const float* __restrict__ dout, int ldd, float* __restrict__ dq, int ldg, float* __restrict__ aw,
+                       float* __restrict__ sw, int B, int P, int Hh) {
+  const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (wid >= B * P * Hh) return;
+  const int head = wid % Hh, bq = wid / Hh, b = bq / P, i = bq % P;
+  float qr[D], gr[D];
+#pragma unroll
+  for (int d = 0; d < D; d += 4) {
+    const float4 a = ldg4(q + (size_t)bq * ldq + head * D + d), c = ldg4(dout + (size_t)bq * ldd + head * D + d);
+    qr[d] = a.x; qr[d + 1] = a.y; qr[d + 2] = a.z; qr[d + 3] = a.w;
+    gr[d] = c.x; gr[d + 1] = c.y; gr[d + 2] = c.z; gr[d + 3] = c.w;
+  }
+  constexpr int MAXK = 16;  // P <= 512
+  float sc[MAXK], dav[MAXK];
+  float m = -INFINITY;
+#pragma unroll
+  for (int n = 0; n < MAXK; ++n) {
+    const int j = n * 32 + lane;
+    sc[n] = -INFINITY;
+    dav[n] = 0.f;
+    if (j < P) {
+      const float* kr = k + (size_t)(b * P + j) * ldk + head * D;
+      const float* vr = v + (size_t)(b * P + j) * ldv + head * D;
+      float s = 0.f, da = 0.f;
+#pragma unroll
+      for (int d = 0; d < D; d += 4) {
+        const float4 a = ldg4(kr + d), c = ldg4(vr + d);
+        s += qr[d] * a.x + qr[d + 1] * a.y + qr[d + 2] * a.z + qr[d + 3] * a.w;
+        da += gr[d] * c.x + gr[d + 1] * c.y + gr[d + 2] * c.z + gr[d + 3] * c.w;
+      }
+      sc[n] = s;
+      dav[n] = da;
+      m = fmaxf(m, s);
+    }
+  }
+  m = warp_max(m);
+  float l = 0.f;
+#pragma unroll
+  for (int n = 0; n < MAXK; ++n) {
+    sc[n] = n * 32 + lane < P ? expf(sc[n] - m) : 0.f;
+    l += sc[n];
+  }
+  const float inv = 1.f / warp_sum(l);
+  float dsum = 0.f;
+#pragma unroll
+  for (int n = 0; n < MAXK; ++n) {
+    sc[n] *= inv;
+    dsum += sc[n] * dav[n];
+  }
+  dsum = warp_sum(dsum);
+  float acc[D];
+#pragma unroll
+  for (int d = 0; d < D; ++d) acc[d] = 0.f;
+  const size_t col = ((size_t)(b * Hh + head) * P) * P + i;      // [b, head, j, i]
+#pragma unroll
+  for (int n = 0; n < MAXK; ++n) {
+    const int j = n * 32 + lane;
+    if (j < P) {
+      const float ds = sc[n] * (dav[n] - dsum);
+      aw[col + (size_t)j * P] = sc[n];
+      sw[col + (size_t)j * P] = ds;
+      const float* kr = k + (size_t)(b * P + j) * ldk + head * D;
+#pragma unroll
+      for (int d = 0; d < D; d += 4) {
+        const float4 a = ldg4(kr + d);
+        acc[d] += ds * a.x; acc[d + 1] += ds * a.y; acc[d + 2] += ds * a.z; acc[d + 3] += ds * a.w;
+      }
+    }
+  }
+#pragma unroll
+  for (int d = 0; d < D; ++d) {
+    const float a = warp_sum(acc[d]);
+    if (lane == d) dq[(size_t)bq * ldg + head * D + d] = a;
+  }
+}
+
+template <int D>
+__global__ void __launch_bounds__(256)
+mha_small_bwd_kv_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ dout, int ldd,
+                        const float* __restrict__ aw, const float* __restrict__ sw, float* __restrict__ dk,
+                        float* __restrict__ dv, int ldg, int B, int P, int Hh) {
+  const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (wid >= B * P * Hh) return;
+  const int head = wid % Hh, bj = wid / Hh, b = bj / P, j = bj % P;
+  const float* ar = aw + ((size_t)(b * Hh + head) * P + j) * P;
+  const float* sr = sw + ((size_t)(b * Hh + head) * P + j) * P;
+  float ak[D], av[D];
+#pragma unroll
+  for (int d = 0; d < D; ++d) ak[d] = av[d] = 0.f;
+  for (int i = lane; i < P; i += 32) {
+    const float a = ar[i], ds = sr[i];
+    const float* qr = q + (size_t)(b * P + i) * ldq + head * D;
+    const float* gr = dout + (size_t)(b * P + i) * ldd + head * D;
+#pragma unroll
+    for (int d = 0; d < D; d += 4) {
+      const float4 x = ldg4(qr + d), y = ldg4(gr + d);
+      ak[d] += ds * x.x; ak[d + 1] += ds * x.y; ak[d + 2] += ds * x.z; ak[d + 3] += ds * x.w;
+      av[d] += a * y.x; av[d + 1] += a * y.y; av[d + 2] += a * y.z; av[d + 3] += a * y.w;
+    }
+  }
+#pragma unroll
+  for (int d = 0; d < D; ++d) {
+    const float x = warp_sum(ak[d]), y = warp_sum(av[d]);
+    if (lane == d) {
+      dk[(size_t)bj * ldg + head * D + d] = x;
+      dv[(size_t)bj * ldg + head * D + d] = y;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Query x BEV cross attention (decoder_utils.py:101-103,466-488): P queries x HW keys, Hh heads of D=16.
 // kv [B*HW, 2*C]: projected keys (cols [0,C)) and values (cols [C,2C)).  Split over key chunks
@@ -1253,6 +1371,24 @@ int di_mha_small_f32(const float* q, int ldq, const float* k, int ldk, const flo
   mha_small_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, onbits, win, B, P, heads,
                                                               nullptr, 0, 1);
   DI_CHECK_LAUNCH("di_mha_small_f32");
+  return DI_OK;
+}
+
+// Backward of di_mha_small_f32 without group masks: dout [B*P, ldd] -> dq / dk / dv rows [B*P, ldg] (e.g. the three
+// column blocks of one [B*P, 3C] gradient); work: float [2 * B * heads * P * P].
+int di_mha_small_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout, int ldd,
+                         float* dq, float* dk, float* dv, int ldg, float* work, int B, int P, int heads, int head_dim,
+                         cudaStream_t stream) {
+  DI_CHECK_ARG(q && k && v && dout && dq && dk && dv && work && B > 0 && P > 0 && heads > 0 && head_dim == 16 && P <= 512,
+               "di_mha_small_bwd_f32: unsupported shape (head_dim=%d P=%d)", head_dim, P);
+  DI_CHECK_ARG(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldd % 4 == 0, "di_mha_small_bwd_f32: strides must be multiples of 4");
+  const int warps = B * P * heads;
+  float* aw = work;
+  float* sw = work + (size_t)B * heads * P * P;
+  mha_small_bwd_q_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, ldg, aw, sw, B, P, heads);
+  DI_CHECK_LAUNCH("di_mha_small_bwd_f32");
+  mha_small_bwd_kv_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, dout, ldd, aw, sw, dk, dv, ldg, B, P, heads);
+  DI_CHECK_LAUNCH("di_mha_small_bwd_f32 (keys)");
   return DI_OK;
 }
 

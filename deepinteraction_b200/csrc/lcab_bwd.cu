@@ -215,6 +215,54 @@ __global__ void col_sum_final_kernel(const float* __restrict__ part, int nblk, i
   out[c] = (float)s;
 }
 
+// LayerNorm backward over [M, C] rows, one warp per row (C <= 512): y = (z - mean) rstd gamma + beta ->
+// dz = rstd (gamma dy - mean(gamma dy) - xhat mean(gamma dy xhat)); prod = dy xhat (its column sums are d gamma)
+__global__ void __launch_bounds__(256)
+ln_bwd_kernel(const float* __restrict__ dy, int ldy, const float* __restrict__ z, int ldz, const float* __restrict__ gamma,
+              float* __restrict__ dz, int lddz, float* __restrict__ prod, int M, int C, float eps) {
+  const int row = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (row >= M) return;
+  constexpr int NV = 16;
+  float zv[NV], gv[NV];
+  float s = 0.f;
+#pragma unroll
+  for (int n = 0; n < NV; ++n) {
+    const int c = n * 32 + lane;
+    zv[n] = c < C ? z[(size_t)row * ldz + c] : 0.f;
+    s += zv[n];
+  }
+  const float mean = warp_sum(s) / (float)C;
+  float var = 0.f;
+#pragma unroll
+  for (int n = 0; n < NV; ++n) {
+    const int c = n * 32 + lane;
+    const float d = c < C ? zv[n] - mean : 0.f;
+    var += d * d;
+  }
+  const float rstd = 1.f / sqrtf(warp_sum(var) / (float)C + eps);
+  float s1 = 0.f, s2 = 0.f;
+#pragma unroll
+  for (int n = 0; n < NV; ++n) {
+    const int c = n * 32 + lane;
+    gv[n] = 0.f;
+    if (c < C) {
+      const float g = dy[(size_t)row * ldy + c];
+      zv[n] = (zv[n] - mean) * rstd;                   // xhat
+      prod[(size_t)row * C + c] = g * zv[n];
+      gv[n] = g * gamma[c];
+      s1 += gv[n];
+      s2 += gv[n] * zv[n];
+    }
+  }
+  s1 = warp_sum(s1) / (float)C;
+  s2 = warp_sum(s2) / (float)C;
+#pragma unroll
+  for (int n = 0; n < NV; ++n) {
+    const int c = n * 32 + lane;
+    if (c < C) dz[(size_t)row * lddz + c] = (gv[n] - s1 - zv[n] * s2) * rstd;
+  }
+}
+
 // out[n, y, x, :] = in[n, y + dy, x + dx, :] (zero outside the map): the shifted copies behind the weight gradient of a
 // 3x3 convolution (dW[co, tap, ci] = sum_p dY[p, co] X[p + tap, ci])
 __global__ void shift_map_kernel(const float4* __restrict__ in, float4* __restrict__ out, int N, int H, int W, int C4, int dy,
@@ -324,6 +372,24 @@ int di_col_sum_f32(const float* x, int ld, long long M, int C, float* work, floa
   col_sum_part_kernel<<<dim3(nblk, di_cdiv(C, 256)), 256, 0, stream>>>(x, ld, M, C, work);
   col_sum_final_kernel<<<di_cdiv(C, 128), 128, 0, stream>>>(work, nblk, C, out);
   DI_CHECK_LAUNCH("di_col_sum_f32");
+  return DI_OK;
+}
+
+// Backward of y = LayerNorm(z) (gamma, beta) over [M, C] rows, C <= 512: dy -> dz, dgamma, dbeta (fixed-order column sums,
+// as di_col_sum_f32); work: float [M * C + 256 * C].
+int di_ln_bwd_f32(const float* dy, int ldy, const float* z, int ldz, const float* gamma, float* dz, int lddz, float* dgamma,
+                  float* dbeta, float* work, int M, int C, float eps, cudaStream_t stream) {
+  DI_CHECK_ARG(dy && z && gamma && dz && dgamma && dbeta && work && M > 0 && C > 0 && C <= 512, "di_ln_bwd_f32: bad argument");
+  float* prod = work;
+  float* part = work + (size_t)M * C;
+  ln_bwd_kernel<<<di_cdiv(M, 8), 256, 0, stream>>>(dy, ldy, z, ldz, gamma, dz, lddz, prod, M, C, eps);
+  DI_CHECK_LAUNCH("di_ln_bwd_f32");
+  const int nblk = M < 256 ? M : 256;
+  col_sum_part_kernel<<<dim3(nblk, di_cdiv(C, 256)), 256, 0, stream>>>(prod, C, M, C, part);
+  col_sum_final_kernel<<<di_cdiv(C, 128), 128, 0, stream>>>(part, nblk, C, dgamma);
+  col_sum_part_kernel<<<dim3(nblk, di_cdiv(C, 256)), 256, 0, stream>>>(dy, ldy, M, C, part);
+  col_sum_final_kernel<<<di_cdiv(C, 128), 128, 0, stream>>>(part, nblk, C, dbeta);
+  DI_CHECK_LAUNCH("di_ln_bwd_f32 (column sums)");
   return DI_OK;
 }
 

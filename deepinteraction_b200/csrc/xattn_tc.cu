@@ -212,9 +212,11 @@ xattn_tc_kernel(const uint32_t* __restrict__ qp, const uint32_t* __restrict__ kp
   }
 }
 
-// merge of the key splits: one warp per (batch, head, query); lanes over the splits
+// merge of the key splits: one warp per (batch, head, query); lanes over the splits.  lse (optional, [B, Hh, P]): the
+// row log-sum-exp M + log L of the logits, which the backward (xattn_bwd.cu) needs to recompute the probabilities
 __global__ void __launch_bounds__(256)
-xattn_combine_kernel(const float* __restrict__ part, float* __restrict__ out, int B, int P, int C, int Hh, int nsplit) {
+xattn_combine_kernel(const float* __restrict__ part, float* __restrict__ out, float* __restrict__ lse, int B, int P, int C,
+                     int Hh, int nsplit) {
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (wid >= B * Hh * P) return;
   const int qi = wid % P, head = (wid / P) % Hh, b = wid / (P * Hh);
@@ -241,6 +243,7 @@ xattn_combine_kernel(const float* __restrict__ part, float* __restrict__ out, in
     if (lane == d) mine = a * inv;
   }
   if (lane < 16) out[(size_t)(b * P + qi) * C + head * 16 + lane] = mine;
+  if (lse && lane == 0) lse[(size_t)(b * Hh + head) * P + qi] = M + logf(L);
 }
 
 // bf16 planes of fp32 rows: hi = bf16(x), mid = bf16(x - hi), lo = bf16(x - hi - mid); a plane holds 128 channels as 64
@@ -317,25 +320,26 @@ int di_xattn_tc_splits(int B, int HW) {
   return n;
 }
 
-// q [B*P, 192 words], k [B*HW, 192 words], v [B*HW, 128 words]: the planes of di_attn_planes_f32; part: workspace
-// (di_xattn_tc_splits), out [B*P, 128] fp32.  8 heads x 16 channels.
-int di_xattn_tc_f32(const void* q, const void* k, const void* v, float* part, float* out, int B, int P, int HW, int heads,
-                    cudaStream_t stream) {
-  DI_CHECK_ARG(q && k && v && part && out && B > 0 && P > 0 && HW > 0, "di_xattn_tc_f32: bad argument");
+}  // extern "C"
+
+namespace {
+int xattn_tc_run(const char* name, const void* q, const void* k, const void* v, float* part, float* out, float* lse, int B,
+                 int P, int HW, int heads, cudaStream_t stream) {
+  DI_CHECK_ARG(q && k && v && part && out && B > 0 && P > 0 && HW > 0, "%s: bad argument", name);
   if (heads != 8 || P > 256) {
-    di_set_error("di_xattn_tc_f32: supported configuration is 8 heads x 16 channels, P <= 256 (got heads=%d P=%d)", heads, P);
+    di_set_error("%s: supported configuration is 8 heads x 16 channels, P <= 256 (got heads=%d P=%d)", name, heads, P);
     return DI_ERR_UNSUPPORTED;
   }
-  DI_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "di_xattn_tc_f32: operands must be 16-byte aligned");
+  DI_CHECK_ARG((((uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "%s: operands must be 16-byte aligned", name);
   int devid = 0;
   cudaGetDevice(&devid);
   if (devid < 0 || devid >= 64) {
-    di_set_error("di_xattn_tc_f32: device ordinal %d not supported", devid);
+    di_set_error("%s: device ordinal %d not supported", name, devid);
     return DI_ERR_UNSUPPORTED;
   }
   if (!g_xt_attr[devid]) {
     if (cudaFuncSetAttribute(xattn_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, XT_SMEM) != cudaSuccess) {
-      di_set_error("di_xattn_tc_f32: cannot reserve %d bytes of shared memory", XT_SMEM);
+      di_set_error("%s: cannot reserve %d bytes of shared memory", name, XT_SMEM);
       return DI_ERR_LAUNCH;
     }
     g_xt_attr[devid] = true;
@@ -351,10 +355,29 @@ int di_xattn_tc_f32(const void* q, const void* k, const void* v, float* part, fl
   xattn_tc_kernel<<<dim3(p.nsplit, mtiles, B), XT_THREADS, XT_SMEM, stream>>>(static_cast<const uint32_t*>(q),
                                                                             static_cast<const uint32_t*>(k),
                                                                             static_cast<const uint32_t*>(v), p);
-  DI_CHECK_LAUNCH("di_xattn_tc_f32");
-  xattn_combine_kernel<<<di_cdiv((long long)B * heads * P, 8), 256, 0, stream>>>(part, out, B, P, heads * 16, heads, p.nsplit);
-  DI_CHECK_LAUNCH("di_xattn_tc_f32 (combine)");
+  DI_CHECK_LAUNCH(name);
+  xattn_combine_kernel<<<di_cdiv((long long)B * heads * P, 8), 256, 0, stream>>>(part, out, lse, B, P, heads * 16, heads,
+                                                                                 p.nsplit);
+  DI_CHECK_LAUNCH(name);
   return DI_OK;
+}
+}  // namespace
+
+extern "C" {
+
+// q [B*P, 192 words], k [B*HW, 192 words], v [B*HW, 128 words]: the planes of di_attn_planes_f32; part: workspace
+// (di_xattn_tc_splits), out [B*P, 128] fp32.  8 heads x 16 channels.
+int di_xattn_tc_f32(const void* q, const void* k, const void* v, float* part, float* out, int B, int P, int HW, int heads,
+                    cudaStream_t stream) {
+  return xattn_tc_run("di_xattn_tc_f32", q, k, v, part, out, nullptr, B, P, HW, heads, stream);
+}
+
+// The same kernels, plus the row log-sum-exp of the logits: lse [B, heads, P] fp32.  out is bit-identical to
+// di_xattn_tc_f32's.
+int di_xattn_tc_lse_f32(const void* q, const void* k, const void* v, float* part, float* out, float* lse, int B, int P,
+                        int HW, int heads, cudaStream_t stream) {
+  DI_CHECK_ARG(lse, "di_xattn_tc_lse_f32: bad argument");
+  return xattn_tc_run("di_xattn_tc_lse_f32", q, k, v, part, out, lse, B, P, HW, heads, stream);
 }
 
 }  // extern "C"

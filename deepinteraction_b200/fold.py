@@ -107,6 +107,53 @@ def i2p_unfold_grads(mha, dM1, dc1, dM2, dc2):
                 Wv=Wo.T @ dM2, Wo=dM2 @ Wv.T + torch.outer(dc2, bv), bv=Wo.T @ dc2, bo=dbo)
 
 
+def decoder_layer_unfold_consts(layer, num_heads, device, dtype=torch.float32):
+    """Constants of decoder_layer_unfold for one TransformerDecoderLayer (built once per pack): the q-row scale of the
+    in-projections and, per positional MLP, the first convolution's weight and bias minus the BN running mean, the BN
+    1 / sqrt(var + eps) and gamma."""
+    C = layer.self_attn.embed_dim
+    s = float(C // num_heads) ** -0.5
+    u = dict(C=C, s=s, qscale=torch.cat([torch.full((C,), s, dtype=torch.float64), torch.ones(2 * C, dtype=torch.float64)]))
+    for name in ('self_posembed', 'cross_posembed'):
+        seq = getattr(layer, name).position_embedding_head
+        conv, bn = seq[0], seq[1]
+        W0 = _d(conv.weight).reshape(conv.weight.shape[0], -1)
+        u[name] = (W0, _d(conv.bias) - _d(bn.running_mean), 1.0 / torch.sqrt(_d(bn.running_var) + bn.eps), _d(bn.weight))
+    cast = lambda t: t.to(device=device, dtype=dtype) if torch.is_tensor(t) else t
+    return {k: (tuple(cast(x) for x in v) if isinstance(v, tuple) else cast(v)) for k, v in u.items()}
+
+
+def decoder_layer_unfold(u, g):
+    """Chain rule from the gradients of the packed, folded weights of the decoder layer (mmpi pack: 'self_attn',
+    'cross_q', 'cross_kv', 'self_pe', 'cross_pe') to the parameters of the TransformerDecoderLayer, keyed and shaped as
+    in its state_dict.  u: decoder_layer_unfold_consts.  Runs where the tensors are (no host round trip).
+    g: self_in (dW [3C, 2C] of [W_s | W_s] over [query | query_pos_embed], db [3C]), cross_q (dW [C, 2C] of [Wq_s | Wq_s],
+    db [C]), cross_kv (dW [2C, C], db [2C]), self_posembed / cross_posembed (dW1 [C, cin], db1 of the conv + BN fold, dW2
+    [C, C], db2).  W_s has its q rows scaled by head_dim^-0.5 (s); the BN fold is W1 = W0 sc, b1 = (b0 - mean) sc + beta,
+    sc = gamma / sqrt(var + eps)."""
+    C, s = u['C'], u['s']
+    out = {}
+    dWp, db = g['self_in']
+    out['self_attn.in_proj_weight'] = (dWp[:, :C] + dWp[:, C:]) * u['qscale'][:, None]
+    out['self_attn.in_proj_bias'] = db * u['qscale']
+    dWq, dbq = g['cross_q']
+    dWkv, dbkv = g['cross_kv']
+    out['multihead_attn.in_proj_weight'] = torch.cat([(dWq[:, :C] + dWq[:, C:]) * s, dWkv], 0)
+    out['multihead_attn.in_proj_bias'] = torch.cat([dbq * s, dbkv])
+    for name in ('self_posembed', 'cross_posembed'):
+        dW1, db1, dW2, db2 = g[name]
+        W0, b0m, inv, gamma = u[name]
+        sc = gamma * inv
+        pre = name + '.position_embedding_head.'
+        out[pre + '0.weight'] = (dW1 * sc[:, None]).unsqueeze(-1)
+        out[pre + '0.bias'] = db1 * sc
+        out[pre + '1.weight'] = ((dW1 * W0).sum(1) + db1 * b0m) * inv
+        out[pre + '1.bias'] = db1
+        out[pre + '3.weight'] = dW2.unsqueeze(-1)
+        out[pre + '3.bias'] = db2
+    return out
+
+
 def dev(t, device):
     return t.to(torch.float32).contiguous().to(device)
 

@@ -340,6 +340,7 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         h = torch.relu(bev_pos @ w1.reshape(w1.shape[0], -1).t() + b1)
         kpe = h @ fold._d(seq[3].weight)[:, :, 0].t() + fold._d(seq[3].bias)
         pk['cross_kv'] = (w_kv, b_kv, d(kpe @ fold._d(W[C:]).t()))
+        pk['cross_pe'] = dict(pos=d(bev_pos), hidden=d(h), kpe=d(kpe))     # the backward's kk = bev + kpe and kpe's MLP
         pk['cross_out'] = (wo, bo)
         for i in (1, 2, 3):
             pk[f'norm{i}'] = lin(getattr(layer, f'norm{i}'))
@@ -458,22 +459,7 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         # transformer decoder layer
         ops._MODULE[0] = ('TransformerDecoderLayer (query x BEV cross-attn)', F_b + 4 * (2 * C * C + 2 * HW * C),
                           2 * B * HW * C * 2 * C + 4 * B * P * HW * C)
-        pw1, pb1, pw2, pb2 = pk['self_pe']
-        qpe = self._mlp([qpos], pw1, pb1, ops.ACT_RELU, pw2, pb2)
-        w, b, wo, bo = pk['self_attn']
-        qkv = self._mlp([q, qpe], w, b)
-        a = ops.mha_small(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H)
-        q = self._mlp([a], wo, bo, res=q, ln=pk['norm1'])
-        qc = self._mlp([q, qpe], *pk['cross_q'])
-        w_kv, b_kv, ckv = pk['cross_kv']
-        kv = ops.linear([pts_conv.view(B * HW, C)], w_kv, b_kv, res=ckv, res_mod=HW)
-        if ops.can_xattn_tc(P, C, H, B * HW):
-            a = ops.xattn_tc(qc, kv, B, P, HW, H)                   # tensor-core attention kernel (xattn_tc.cu)
-        else:
-            a = ops.cross_attn(qc, kv, B, P, HW, H)
-        q = self._mlp([a], *pk['cross_out'], res=q, ln=pk['norm2'])
-        f1w, f1b, f2w, f2b = pk['ffn']
-        q = self._mlp([q], f1w, f1b, ops.ACT_RELU, f2w, f2b, res=q, ln=pk['norm3'])
+        q = self._layer(pk, q, qpos, pts_conv, B, P)
         ops._MODULE[0] = ('prediction_heads', 0, 0)
         pred = self._pred(pk['pred0'], [q])
         ops.pred_finish(pred, qpos)
@@ -539,6 +525,41 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
                 debug.setdefault('rois', []).append(rois)
         ops._MODULE[0] = None
         return dict(preds=preds, wins=wins, keeps=keeps, qscore=qscore, dense_heatmap=dense_b, labels=labels)
+
+    def _layer(self, pk, q, qpos, bev, B, P, saved=None):
+        """TransformerDecoderLayer (decoder_utils.py:35-113) on query rows: q [B*P, C], qpos [B*P, 2], bev [B, Y, X, C]
+        (pts_conv) -> [B*P, C].  The one implementation of the layer, for the forward schedule and for the eager re-run of
+        backward.decoder_layer_backward.  saved (a dict) selects the re-run: the cross attention then always runs through
+        xattn_tc_lse, so that its output O and row log-sum-exp come from one kernel, and the values the backward needs are
+        stored in `saved`; the returned rows are the same either way."""
+        C, H = self.hidden_channel, self.num_heads
+        HW = bev.shape[1] * bev.shape[2]
+        pw1, pb1, pw2, pb2 = pk['self_pe']
+        qpe = self._mlp([qpos], pw1, pb1, ops.ACT_RELU, pw2, pb2)
+        w, b, wo, bo = pk['self_attn']
+        qkv = self._mlp([q, qpe], w, b)
+        a = ops.mha_small(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H)
+        q1 = self._mlp([a], wo, bo, res=q, ln=pk['norm1'])
+        qc = self._mlp([q1, qpe], *pk['cross_q'])
+        w_kv, b_kv, ckv = pk['cross_kv']
+        kv = ops.linear([bev.view(B * HW, C)], w_kv, b_kv, res=ckv, res_mod=HW)
+        if saved is not None:
+            a2, lse, planes = ops.xattn_tc_lse(qc, kv, B, P, HW, H)
+        elif ops.can_xattn_tc(P, C, H, B * HW):
+            a2 = ops.xattn_tc(qc, kv, B, P, HW, H)                  # tensor-core attention kernel (xattn_tc.cu)
+        else:
+            a2 = ops.cross_attn(qc, kv, B, P, HW, H)
+        q2 = self._mlp([a2], *pk['cross_out'], res=q1, ln=pk['norm2'])
+        f1w, f1b, f2w, f2b = pk['ffn']
+        q3 = self._mlp([q2], f1w, f1b, ops.ACT_RELU, f2w, f2b, res=q2, ln=pk['norm3'])
+        if saved is not None:
+            # pre-norm sums and the hidden rows of the two-layer MLPs, which the fused row kernels do not return
+            f = self._mlp([q2], f1w, f1b, ops.ACT_RELU)
+            saved.update(qpe=qpe, hs=self._mlp([qpos], pw1, pb1, ops.ACT_RELU), qkv=qkv, a1=a,
+                         z1=self._mlp([a], wo, bo, res=q), q1=q1, a2=a2, lse=lse, planes=planes,
+                         z2=self._mlp([a2], *pk['cross_out'], res=q1), q2=q2, f=f, z3=self._mlp([f], f2w, f2b, res=q2),
+                         kk=ops.add_rows_mod(bev.reshape(B * HW, C), pk['cross_pe']['kpe']))
+        return q3
 
     def _to_dict(self, pred, B, P):
         t = pred.view(B, P, self.NP).permute(0, 2, 1)

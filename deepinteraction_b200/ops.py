@@ -840,9 +840,7 @@ def can_xattn_tc(P, C, heads, M_keys):
     return bool(XATTN_TC[0] and USE_TC[0] and C == 128 and heads == 8 and P <= 256 and M_keys >= TC_MIN_M[0])
 
 
-def xattn_tc(q, kv, B, P, HW, heads):
-    """q [B*P, 128] fp32 (pre-scaled queries), kv [B*HW, 256] fp32 (K | V) -> softmax(q k^T) v per head, [B*P, 128] fp32:
-    operand planes (di_attn_planes_f32) + the mma.sync attention kernel + the split merge."""
+def _xattn_planes(q, kv, B, P, HW):
     assert kv.is_contiguous() and kv.shape == (B * HW, 256) and q.shape == (B * P, 128)
     dev_ = q.device
     qp = torch.empty(B * P, 192, device=dev_, dtype=torch.float32)
@@ -851,9 +849,72 @@ def xattn_tc(q, kv, B, P, HW, heads):
     pq, lq = _rows(q)
     _call('di_attn_planes_f32', pq, lq, _ptr(qp), B * P, _ptr(kv), 256, _ptr(kp), _ptr(vp), B * HW, _stream(),
           nbytes=4 * (kv.numel() + kp.numel() + vp.numel()), launches=2)
+    return qp, kp, vp
+
+
+def xattn_tc(q, kv, B, P, HW, heads):
+    """q [B*P, 128] fp32 (pre-scaled queries), kv [B*HW, 256] fp32 (K | V) -> softmax(q k^T) v per head, [B*P, 128] fp32:
+    operand planes (di_attn_planes_f32) + the mma.sync attention kernel + the split merge."""
+    qp, kp, vp = _xattn_planes(q, kv, B, P, HW)
     nsplit = _lib.lib().di_xattn_tc_splits(B, HW)
-    part = torch.empty(B * heads * nsplit * 18 * P, device=dev_, dtype=torch.float32)
-    out = torch.empty(B * P, 128, device=dev_, dtype=torch.float32)
+    part = torch.empty(B * heads * nsplit * 18 * P, device=q.device, dtype=torch.float32)
+    out = torch.empty(B * P, 128, device=q.device, dtype=torch.float32)
     _call('di_xattn_tc_f32', _ptr(qp), _ptr(kp), _ptr(vp), _ptr(part), _ptr(out), B, P, HW, heads, _stream(),
           nbytes=4 * (kp.numel() + vp.numel() + 2 * q.numel()), flops=4 * B * P * HW * 128, launches=2)
     return out
+
+
+def xattn_tc_lse(q, kv, B, P, HW, heads):
+    """xattn_tc plus the row log-sum-exp of the logits: -> (out [B*P, 128] (bit-identical to xattn_tc), lse [B, heads, P],
+    planes (q, k, v operand planes, the inputs of xattn_bwd))."""
+    planes = _xattn_planes(q, kv, B, P, HW)
+    nsplit = _lib.check(_lib.lib().di_xattn_tc_splits(B, HW), 'di_xattn_tc_splits')
+    part = torch.empty(B * heads * nsplit * 18 * P, device=q.device, dtype=torch.float32)
+    out = torch.empty(B * P, 128, device=q.device, dtype=torch.float32)
+    lse = torch.empty(B, heads, P, device=q.device, dtype=torch.float32)
+    _call('di_xattn_tc_lse_f32', *(_ptr(t) for t in planes), _ptr(part), _ptr(out), _ptr(lse), B, P, HW, heads, _stream(),
+          nbytes=4 * (planes[1].numel() + planes[2].numel() + 2 * q.numel()), flops=4 * B * P * HW * 128, launches=2)
+    return out, lse, planes
+
+
+def xattn_bwd(planes, out, lse, dout, B, P, HW, heads, dkv=None):
+    """Gradient of xattn_tc_lse (csrc/xattn_bwd.cu): dout [B*P, 128] -> (dq [B*P, 128] w.r.t. the pre-scaled queries,
+    dkv [B*HW, 256] = dK | dV).  dkv may be given (rows [B*HW, >= 256]); only its first 256 columns are written."""
+    qp, kp, vp = planes
+    dev_ = out.device
+    if dkv is None:
+        dkv = torch.empty(B * HW, 256, device=dev_, dtype=torch.float32)
+    assert dkv.shape[0] == B * HW and dkv.stride(1) == 1 and dkv.stride(0) >= 256
+    pd, ld = _rows(dout)
+    n = _lib.check(_lib.lib().di_xattn_bwd_workspace(B, P, HW), 'di_xattn_bwd_workspace')
+    work = torch.empty(n, device=dev_, dtype=torch.float32)
+    dq = torch.empty(B * P, 128, device=dev_, dtype=torch.float32)
+    _call('di_xattn_bwd_f32', _ptr(qp), _ptr(kp), _ptr(vp), _ptr(out), pd, ld, _ptr(lse), _ptr(work), _ptr(dq), _ptr(dkv),
+          ctypes.c_void_p(dkv.data_ptr() + 128 * 4), dkv.stride(0), B, P, HW, heads, _stream(),
+          nbytes=4 * (kp.numel() + vp.numel() + 2 * B * HW * 128), flops=10 * B * P * HW * 128, launches=3)
+    return dq, dkv
+
+
+def mha_small_bwd(q, k, v, dout, B, P, heads):
+    """Gradient of mha_small without group masks: -> dqkv [B*P, 3C] = dq | dk | dv."""
+    C = q.shape[1]
+    dqkv = torch.empty(B * P, 3 * C, device=q.device, dtype=torch.float32)
+    work = torch.empty(2 * B * heads * P * P, device=q.device, dtype=torch.float32)
+    (pq, lq), (pk, lk), (pv, lv), (pd, ld) = _rows(q), _rows(k), _rows(v), _rows(dout)
+    base = dqkv.data_ptr()
+    _call('di_mha_small_bwd_f32', pq, lq, pk, lk, pv, lv, pd, ld, ctypes.c_void_p(base), ctypes.c_void_p(base + 4 * C),
+          ctypes.c_void_p(base + 8 * C), 3 * C, _ptr(work), B, P, heads, C // heads, _stream(), launches=2)
+    return dqkv
+
+
+def ln_bwd(dy, z, gamma, eps=1e-5):
+    """Backward of y = LayerNorm(z) * gamma + beta over [M, C] rows (z: the pre-norm sum) -> (dz, dgamma, dbeta)."""
+    M, C = z.shape
+    dz = torch.empty(M, C, device=z.device, dtype=torch.float32)
+    dg = torch.empty(C, device=z.device, dtype=torch.float32)
+    db = torch.empty(C, device=z.device, dtype=torch.float32)
+    work = torch.empty(M * C + 256 * C, device=z.device, dtype=torch.float32)
+    (py, ly), (pz, lz) = _rows(dy), _rows(z)
+    _call('di_ln_bwd_f32', py, ly, pz, lz, _ptr(gamma), _ptr(dz), C, _ptr(dg), _ptr(db), _ptr(work), M, C, float(eps), _stream(),
+          nbytes=4 * 4 * M * C, launches=5)
+    return dz, dg, db

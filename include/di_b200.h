@@ -249,6 +249,10 @@ int di_query_init_f32(const float* feat, const int* top, const float* heat, cons
 /* self-attention among the queries of a sample (models/utils/decoder_utils.py:95-99, :745, :826) */
 int di_mha_small_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo,
                      const int* onbits, const int* win, int B, int P, int heads, int head_dim, cudaStream_t stream);
+/* its backward without group masks: dout -> dq, dk, dv rows [B*P, ldg]; work: float [2 * B * heads * P * P]; deterministic */
+int di_mha_small_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout, int ldd,
+                         float* dq, float* dk, float* dv, int ldg, float* work, int B, int P, int heads, int head_dim,
+                         cudaStream_t stream);
 /* query x BEV cross attention (models/utils/decoder_utils.py:101-103, 466-488) */
 int di_cross_attn_f32(const float* q, const float* kv, float* part, float* out, int B, int P, int HW, int C, int heads,
                       int nsplit, cudaStream_t stream);
@@ -361,6 +365,10 @@ int di_win_softmax_bwd_f32(const float* A, const float* dA, float* dS, long long
 /* ReLU backward from the saved output; column sums of a [M, C] matrix (bias gradients; work: float [256 * C]) */
 int di_relu_bwd_f32(const float* dy, const float* y, float* dx, long long n, cudaStream_t stream);
 int di_col_sum_f32(const float* x, int ld, long long M, int C, float* work, float* out, cudaStream_t stream);
+/* backward of y = LayerNorm(z) over [M, C] rows (z = the saved pre-norm sum): dz, dgamma, dbeta (fixed-order column sums);
+ * work: float [M * C + 256 * C] */
+int di_ln_bwd_f32(const float* dy, int ldy, const float* z, int ldz, const float* gamma, float* dz, int lddz, float* dgamma,
+                  float* dbeta, float* work, int M, int C, float eps, cudaStream_t stream);
 /* zero-filled shift of a pixel-major map (weight gradient of the 3x3 shared convolutions) */
 int di_shift_map_f32(const float* in, float* out, int N, int H, int W, int C, int dy, int dx, cudaStream_t stream);
 
@@ -411,6 +419,19 @@ int di_attn_planes_f32(const float* q, int ld_q, void* qplanes, int M, const flo
 int di_xattn_tc_splits(int B, int HW);
 int di_xattn_tc_f32(const void* q, const void* k, const void* v, float* part, float* out, int B, int P, int HW, int heads,
                     cudaStream_t stream);
+/* di_xattn_tc_lse_f32: the same kernels, plus lse [B, heads, P] = the row log-sum-exp of the logits (from the split merge);
+ * out is bit-identical to di_xattn_tc_f32's. */
+int di_xattn_tc_lse_f32(const void* q, const void* k, const void* v, float* part, float* out, float* lse, int B, int P,
+                        int HW, int heads, cudaStream_t stream);
+/* ---- backward of the query x BEV cross attention (xattn_bwd.cu): mma.sync bf16 split on the operand planes, key splits with
+ * dK / dV written once per key and per-split dQ partials merged in a fixed order (no atomics; deterministic).
+ * q / k / v: planes of di_attn_planes_f32; out, lse: outputs of di_xattn_tc_lse_f32; dout [B*P, ld_dout] -> dq [B*P, 128]
+ * (w.r.t. the pre-scaled queries), dk / dv rows [B*HW, ld_dkv]; work: di_xattn_bwd_workspace(B, P, HW) floats.  8 heads x 16
+ * channels, P <= 256. */
+int di_xattn_bwd_workspace(int B, int P, int HW);
+int di_xattn_bwd_f32(const void* q, const void* k, const void* v, const float* out, const float* dout, int ld_dout,
+                     const float* lse, float* work, float* dq, float* dk, float* dv, int ld_dkv, int B, int P, int HW,
+                     int heads, cudaStream_t stream);
 
 #ifdef __cplusplus
 }
