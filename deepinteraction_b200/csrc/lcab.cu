@@ -12,7 +12,7 @@
 // (then v) streams through shared memory in 16-channel chunks with cp.async double buffering;
 // each thread keeps the k*k logits of its query in registers, so logits/probabilities never
 // touch HBM (the reference writes and re-reads 2*N*81*4 bytes per call).
-#include "common.cuh"
+#include "tc_common.cuh"
 
 namespace {
 
@@ -575,17 +575,62 @@ lcab_window_bf16_kernel(const float* __restrict__ q, int ldq, const float* __res
 // epilogue already as bf16 (hi, mid) words (gemm_tc.cu), 4 bytes per value at the value's own position.
 // The two conversion passes, one barrier per stage and the packed-V buffer disappear: stages go straight from
 // cp.async to fragments (LDS.64 for Q/K, ldmatrix.x4.trans for V).
-// PLANAR: q, k, v in the planar format (split kind 3, C = 128: per pixel 64 hi words | 64 mid words).  A 32-channel
-// stage then holds per pixel 16 hi words | 16 mid words; fragments take the hi and mid word of a channel pair from the
-// two halves, and the ldmatrix.trans rows of V are the 8-channel groups of either half.
 // ------------------------------------------------------------------------------------------------
 constexpr int VSTR2 = 36;                                            // V chunk pixel stride: 8 ldmatrix rows -> 32 distinct banks
 
-template <bool PLANAR>
+// Masked softmax over the 81 in-window keys of the warp's two query rows (fragment rows g: query row wy, g + 8: row
+// wy + 1), then P = softmax(S) packed as the bf16 hi / mid A fragments of P V: for halo row r, k = the 16 halo columns
+// wx .. wx+15 (block cb = 0 -> k 0..7, cb = 1 -> 8..15).
+__device__ __forceinline__ void window_softmax(float (&S)[20][4], float scale, int g, int t, uint32_t (&Ph)[10][4],
+                                               uint32_t (&Pm)[10][4]) {
+  float m0 = -INFINITY, m1 = -INFINITY;
+#pragma unroll
+  for (int b = 0; b < 20; ++b) {
+    const int r = b >> 1, cb = b & 1;
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      const int d = cb * 8 + 2 * t + j - g;               // key column - query column + 4
+      const bool colok = d >= 0 && d <= 8;
+      S[b][j] = (colok && r <= 8) ? S[b][j] * scale : -INFINITY;
+      S[b][2 + j] = (colok && r >= 1) ? S[b][2 + j] * scale : -INFINITY;
+      m0 = fmaxf(m0, S[b][j]);
+      m1 = fmaxf(m1, S[b][2 + j]);
+    }
+  }
+  m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
+  m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
+  m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
+  m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
+  float s0 = 0.f, s1 = 0.f;
+#pragma unroll
+  for (int b = 0; b < 20; ++b)
+#pragma unroll
+    for (int j = 0; j < 2; ++j) {
+      S[b][j] = expf(S[b][j] - m0);            // exp(-inf) = 0 for out-of-window entries
+      S[b][2 + j] = expf(S[b][2 + j] - m1);
+      s0 += S[b][j];
+      s1 += S[b][2 + j];
+    }
+  s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
+  s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
+  s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
+  s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
+  const float i0 = 1.f / s0, i1 = 1.f / s1;
+#pragma unroll
+  for (int r = 0; r < 10; ++r)
+#pragma unroll
+    for (int cb = 0; cb < 2; ++cb) {
+      const uint2 lo = split_bf16x2(S[r * 2 + cb][0] * i0, S[r * 2 + cb][1] * i0);   // row g
+      const uint2 hi = split_bf16x2(S[r * 2 + cb][2] * i1, S[r * 2 + cb][3] * i1);   // row g + 8
+      Ph[r][cb * 2] = lo.x; Pm[r][cb * 2] = lo.y;
+      Ph[r][cb * 2 + 1] = hi.x; Pm[r][cb * 2 + 1] = hi.y;
+    }
+}
+
 __global__ void __launch_bounds__(256, 1)
 lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
-                        const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
-                        float scale) {
+                       const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
+                       float scale) {
   extern __shared__ __align__(16) float smem[];   // [2][BSTAGE_WORDS]: K,Q chunk (pixel stride 40 words) or V chunk (36)
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
@@ -601,14 +646,11 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
     const int c0 = (is_k ? stage : stage - nchunk) * MCH;
     float* dst = smem + (stage & 1) * BSTAGE_WORDS;
     const int pstr = is_k ? BSTR : VSTR2;
-    // source word of the stage's 16-byte piece c4: kind 1 / 2 keep a channel's position; planar: 4 pieces of hi
-    // words (c0 / 2 ..), then 4 pieces of mid words (64 + c0 / 2 ..)
-    auto src_word = [&](int c4) { return PLANAR ? (c4 < 4 ? c0 / 2 + c4 * 4 : 64 + c0 / 2 + (c4 - 4) * 4) : c0 + c4 * 4; };
     for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
       int px = i / (MCH / 4), c4 = i % (MCH / 4);
       int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
       bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
-      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + src_word(c4) : src;
+      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
       cp_async16(dst + px * pstr + c4 * 4, gp, ok);
     }
     if (is_k) {
@@ -617,15 +659,11 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
         int px = i / (MCH / 4), c4 = i % (MCH / 4);
         int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
         bool ok = gy < H && gx < W;
-        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + src_word(c4) : q;
+        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
         cp_async16(qd + px * BSTR + c4 * 4, gp, ok);
       }
     }
     cp_async_commit();
-  };
-  // (hi, mid) words of channel pair j of a pixel row in a K / Q stage
-  auto pair_at = [](const uint32_t* row, int j) -> uint2 {
-    return PLANAR ? make_uint2(row[j], row[16 + j]) : *reinterpret_cast<const uint2*>(row + 2 * j);
   };
 
   const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
@@ -652,10 +690,10 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
       for (int ks = 0; ks < MCH / 16; ++ks) {
         uint32_t ah[4], am[4];
         {
-          const uint2 a0 = pair_at(qw + g * BSTR, ks * 8 + t);
-          const uint2 a1 = pair_at(qw + (MQ_COLS + g) * BSTR, ks * 8 + t);
-          const uint2 a2 = pair_at(qw + g * BSTR, ks * 8 + t + 4);
-          const uint2 a3 = pair_at(qw + (MQ_COLS + g) * BSTR, ks * 8 + t + 4);
+          const uint2 a0 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t) * 2);
+          const uint2 a1 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t) * 2);
+          const uint2 a2 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t + 4) * 2);
+          const uint2 a3 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t + 4) * 2);
           ah[0] = a0.x; am[0] = a0.y; ah[1] = a1.x; am[1] = a1.y;
           ah[2] = a2.x; am[2] = a2.y; ah[3] = a3.x; am[3] = a3.y;
         }
@@ -667,8 +705,8 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
 #pragma unroll
           for (int u = 0; u < 4; ++u) {
             const uint32_t* kp = kw + ((wy + 2 * r2 + (u >> 1)) * MT_COLS + wx + (u & 1) * 8 + g) * BSTR;
-            b0[u] = pair_at(kp, ks * 8 + t);
-            b1[u] = pair_at(kp, ks * 8 + t + 4);
+            b0[u] = *reinterpret_cast<const uint2*>(kp + 2 * (ks * 8 + t));
+            b1[u] = *reinterpret_cast<const uint2*>(kp + 2 * (ks * 8 + t + 4));
           }
 #pragma unroll
           for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
@@ -678,63 +716,16 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
           for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
         }
       }
-      if (stage == nchunk - 1) {
-        // ---------------- masked softmax over the 81 in-window keys ----------------
-        float m0 = -INFINITY, m1 = -INFINITY;   // fragment rows g (query row wy) and g+8 (query row wy+1)
-#pragma unroll
-        for (int b = 0; b < 20; ++b) {
-          const int r = b >> 1, cb = b & 1;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int d = cb * 8 + 2 * t + j - g;               // key column - query column + 4
-            const bool colok = d >= 0 && d <= 8;
-            S[b][j] = (colok && r <= 8) ? S[b][j] * scale : -INFINITY;
-            S[b][2 + j] = (colok && r >= 1) ? S[b][2 + j] * scale : -INFINITY;
-            m0 = fmaxf(m0, S[b][j]);
-            m1 = fmaxf(m1, S[b][2 + j]);
-          }
-        }
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int b = 0; b < 20; ++b)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            S[b][j] = expf(S[b][j] - m0);            // exp(-inf) = 0 for out-of-window entries
-            S[b][2 + j] = expf(S[b][2 + j] - m1);
-            s0 += S[b][j];
-            s1 += S[b][2 + j];
-          }
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        const float i0 = 1.f / s0, i1 = 1.f / s1;
-        // A fragments of P V for halo row r: k = the 16 halo columns wx .. wx+15 (block cb=0 -> k 0..7, cb=1 -> 8..15)
-#pragma unroll
-        for (int r = 0; r < 10; ++r)
-#pragma unroll
-          for (int cb = 0; cb < 2; ++cb) {
-            const uint2 lo = split_bf16x2(S[r * 2 + cb][0] * i0, S[r * 2 + cb][1] * i0);   // row g
-            const uint2 hi = split_bf16x2(S[r * 2 + cb][2] * i1, S[r * 2 + cb][3] * i1);   // row g + 8
-            Ph[r][cb * 2] = lo.x; Pm[r][cb * 2] = lo.y;
-            Ph[r][cb * 2 + 1] = hi.x; Pm[r][cb * 2 + 1] = hi.y;
-          }
-      }
+      if (stage == nchunk - 1) window_softmax(S, scale, g, t, Ph, Pm);
     } else {
       // ---------------- O[chunk] = P V[chunk] ----------------
-      // V arrives pre-split in 8-channel groups [4 hi words | 4 mid words] (planar: hi groups in words 0..15, mid groups
-      // in 16..31); ldmatrix.trans turns the [key][channel] rows into the (k = key pair, n = channel) B fragments:
-      // matrices 0/1 = keys 0-7 / 8-15 hi, 2/3 = the mid parts.
-      constexpr int MID_OFF = PLANAR ? 16 : 4, NB_STEP = PLANAR ? 4 : 8;
+      // V arrives pre-split in 8-channel groups [4 hi words | 4 mid words]; ldmatrix.trans turns the [key][channel]
+      // rows into the (k = key pair, n = channel) B fragments: matrices 0/1 = keys 0-7 / 8-15 hi, 2/3 = the mid parts.
       float O[MCH / 8][4];
 #pragma unroll
       for (int nb = 0; nb < MCH / 8; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
       const uint32_t vbase = (uint32_t)__cvta_generic_to_shared(buf) +
-                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * MID_OFF) * 4);
+                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * 4) * 4);
 #pragma unroll
       for (int r = 0; r < 10; ++r) {
         uint32_t bh0[MCH / 8], bh1[MCH / 8], bm0[MCH / 8], bm1[MCH / 8];
@@ -742,7 +733,7 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
         for (int nb = 0; nb < MCH / 8; ++nb)
           asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
                        : "=r"(bh0[nb]), "=r"(bh1[nb]), "=r"(bm0[nb]), "=r"(bm1[nb])
-                       : "r"(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * NB_STEP) * 4)));
+                       : "r"(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * 8) * 4)));
 #pragma unroll
         for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Pm[r], bh0[nb], bh1[nb]);
 #pragma unroll
@@ -767,6 +758,205 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
     }
     __syncthreads();
   }
+}
+
+// ------------------------------------------------------------------------------------------------
+// PLANAR operands (split kind 3, C = 128: per pixel 64 hi words | 64 mid words; lcab_proj.cu writes them): the same
+// per-warp math as the kernel above -- 2 x 8 query patch and 10 x 16 key region per warp, k16 steps over 32-channel
+// chunks, the three split products in the order mid.hi, hi.mid, hi.hi, the same softmax and P V key grouping -- so the
+// results are bit-identical to it on the same hi / mid words.  What differs is how the operands arrive:
+//   persistent grid: min(tiles, SMs) CTAs walk the 8 x 16 query tiles with a static stride in (image, band, column)
+//     order (no atomic tile counter: graphs on concurrent streams must not share scheduler state);
+//   TMA: per stage one elected thread loads the hi and the mid plane of the 32-channel chunk -- K (16 x 24 halo) and Q
+//     (8 x 16), or V -- as boxes of a 4-D tensor map {word, x, y, image}; out-of-image pixels (negative or too large
+//     coordinates) arrive zero-filled, which gives the reference's out-of-image rule as the padded kernels' halo does;
+//   a 3-slot full / empty mbarrier ring over the 8 stages of a tile (4 K+Q, 4 V) and across tiles, so the next
+//     tile's first stages load while the current one runs its softmax, P V and stores.  The producer is thread 0, which
+//     refills a slot once all 8 warps have released it; no block-wide barrier is left in the loop;
+//   64-byte swizzle: a plane is rows of 64 bytes (16 words of one pixel); TMA stores 16-byte chunk c of row R at chunk
+//     c ^ ((R >> 1) & 3).  Every fragment load reads 8 consecutive pixels of a row block starting at a multiple of 8,
+//     so the XOR is a per-lane constant, and the 8 pixels cover all 32 banks (R & 1 picks the bank half, the XOR the
+//     quarter): Q / K loads and the V ldmatrix rows are conflict-free.
+// ------------------------------------------------------------------------------------------------
+constexpr int TC_KV_PLANE = MT_ROWS * MT_COLS * 64;                  // 24576 B: one half (hi or mid) of a 16 x 24 halo chunk
+constexpr int TC_Q_PLANE = MQ_ROWS * MQ_COLS * 64;                   // 8192 B
+constexpr int TC_SLOT = 2 * TC_KV_PLANE + 2 * TC_Q_PLANE;            // 64 KB: K hi | K mid | Q hi | Q mid, or V hi | V mid
+constexpr int TC_S = 3;                                              // ring slots
+constexpr int TC_SMEM_BYTES = TC_S * TC_SLOT + 1024 /*alignment*/ + 64 /*barriers*/;
+static_assert(TC_SMEM_BYTES <= 232448, "lcab_window_tc exceeds the 227 KB shared-memory limit");
+
+__global__ void __launch_bounds__(256, 1)
+lcab_window_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_constant__ CUtensorMap mapK,
+                      const __grid_constant__ CUtensorMap mapV, float* __restrict__ out, int ldo, int H, int W, int bands,
+                      int cols, int tiles, float scale) {
+  extern __shared__ uint8_t smem_raw[];
+  const uint32_t base = (tc::smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint8_t* base_ptr = smem_raw + (base - tc::smem_u32(smem_raw));
+  const uint32_t bars = base + TC_S * TC_SLOT;
+  auto full = [&](int s) { return bars + 8u * s; };
+  auto empty = [&](int s) { return bars + 8u * (TC_S + s); };
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int per_image = bands * cols;
+
+  if (tid == 0) {
+    for (int s = 0; s < TC_S; ++s) {
+      tc::mbar_init(full(s), 1);
+      tc::mbar_init(empty(s), 8);                    // one arrival per warp
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+
+  // ---- producer (thread 0): the next stage to load is stage pj of tile ptile, the pit-th stage of this CTA
+  int ptile = blockIdx.x, pj = 0, pit = 0;
+  auto produce = [&]() {
+    if (ptile >= tiles) return;
+    const int s = pit % TC_S;
+    if (pit >= TC_S) tc::mbar_wait(empty(s), (pit / TC_S - 1) & 1);
+    const int n = ptile / per_image, rem = ptile - n * per_image;
+    const int y0 = (rem / cols) * MQ_ROWS, x0 = (rem % cols) * MQ_COLS;
+    const uint32_t dst = base + s * TC_SLOT;
+    const int c = (pj & 3) * 16;                     // hi words of the chunk; its mid words are at 64 + c
+    if (pj < 4) {
+      tc::mbar_expect_tx(full(s), TC_SLOT);
+      tc::tma_load_4d(dst, &mapK, full(s), c, x0 - 4, y0 - 4, n);
+      tc::tma_load_4d(dst + TC_KV_PLANE, &mapK, full(s), 64 + c, x0 - 4, y0 - 4, n);
+      tc::tma_load_4d(dst + 2 * TC_KV_PLANE, &mapQ, full(s), c, x0, y0, n);
+      tc::tma_load_4d(dst + 2 * TC_KV_PLANE + TC_Q_PLANE, &mapQ, full(s), 64 + c, x0, y0, n);
+    } else {
+      tc::mbar_expect_tx(full(s), 2 * TC_KV_PLANE);
+      tc::tma_load_4d(dst, &mapV, full(s), c, x0 - 4, y0 - 4, n);
+      tc::tma_load_4d(dst + TC_KV_PLANE, &mapV, full(s), 64 + c, x0 - 4, y0 - 4, n);
+    }
+    ++pit;
+    if (++pj == 8) {
+      pj = 0;
+      ptile += gridDim.x;
+    }
+  };
+  if (tid == 0) {
+    produce();
+    produce();
+  }
+
+  // ---- consumers: all 8 warps
+  int slot = 0;
+  uint32_t phase = 0;
+  auto release = [&]() {                             // this warp is done reading the slot
+    __syncwarp();
+    if (lane == 0) tc::mbar_arrive(empty(slot));
+    if (++slot == TC_S) {
+      slot = 0;
+      phase ^= 1u;
+    }
+  };
+  const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
+  // byte offset of word t of 16-byte chunk c in pixel g of an 8-aligned row block: fl ^ (c << 4)
+  const uint32_t fl = g * 64 + (((g >> 1) & 3) << 4) + t * 4;
+  // ldmatrix row of lane l: pixel l & 15 of the block (keys 0-7 / 8-15), hi plane for l < 16, mid plane above
+  const uint32_t vl = (lane >> 4) * TC_KV_PLANE + (lane & 15) * 64 + (((lane >> 1) & 3) << 4);
+  auto ld32 = [&](uint32_t off) { return *reinterpret_cast<const uint32_t*>(base_ptr + off); };
+
+  for (int tile = blockIdx.x; tile < tiles; tile += gridDim.x) {
+    const int n = tile / per_image, rem = tile - n * per_image;
+    const int y0 = (rem / cols) * MQ_ROWS, x0 = (rem % cols) * MQ_COLS;
+    float S[20][4];
+#pragma unroll
+    for (int b = 0; b < 20; ++b) S[b][0] = S[b][1] = S[b][2] = S[b][3] = 0.f;
+    uint32_t Ph[10][4], Pm[10][4];
+
+#pragma unroll 1
+    for (int j = 0; j < 4; ++j) {
+      // ---------------- S += Q[chunk] K[chunk]^T ----------------
+      if (tid == 0) produce();
+      tc::mbar_wait(full(slot), phase);
+      const uint32_t kb = slot * TC_SLOT + (wy * MT_COLS + wx) * 64;
+      const uint32_t qb = slot * TC_SLOT + 2 * TC_KV_PLANE + (wy * MQ_COLS + wx) * 64;
+#pragma unroll
+      for (int ks = 0; ks < 2; ++ks) {
+        const uint32_t f0 = fl ^ ((2 * ks) << 4), f1 = fl ^ ((2 * ks + 1) << 4);   // words ks*8 + t, ks*8 + t + 4
+        uint32_t ah[4], am[4];
+        ah[0] = ld32(qb + f0);                       am[0] = ld32(qb + TC_Q_PLANE + f0);
+        ah[1] = ld32(qb + MQ_COLS * 64 + f0);        am[1] = ld32(qb + TC_Q_PLANE + MQ_COLS * 64 + f0);
+        ah[2] = ld32(qb + f1);                       am[2] = ld32(qb + TC_Q_PLANE + f1);
+        ah[3] = ld32(qb + MQ_COLS * 64 + f1);        am[3] = ld32(qb + TC_Q_PLANE + MQ_COLS * 64 + f1);
+#pragma unroll
+        for (int r2 = 0; r2 < 5; ++r2) {
+          uint2 b0[4], b1[4];                        // (hi, mid) of the B fragment's two k halves
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            const uint32_t kp = kb + ((2 * r2 + (u >> 1)) * MT_COLS + (u & 1) * 8) * 64;
+            b0[u] = make_uint2(ld32(kp + f0), ld32(kp + TC_KV_PLANE + f0));
+            b1[u] = make_uint2(ld32(kp + f1), ld32(kp + TC_KV_PLANE + f1));
+          }
+#pragma unroll
+          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
+#pragma unroll
+          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].y, b1[u].y);
+#pragma unroll
+          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
+        }
+      }
+      release();
+      if (j == 3) window_softmax(S, scale, g, t, Ph, Pm);
+    }
+
+#pragma unroll 1
+    for (int j = 0; j < 4; ++j) {
+      // ---------------- O[chunk] = P V[chunk] ----------------
+      if (tid == 0) produce();
+      tc::mbar_wait(full(slot), phase);
+      float O[4][4];
+#pragma unroll
+      for (int nb = 0; nb < 4; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
+      const uint32_t vb = base + slot * TC_SLOT + (wy * MT_COLS + wx) * 64;
+#pragma unroll
+      for (int r = 0; r < 10; ++r) {
+        uint32_t bh0[4], bh1[4], bm0[4], bm1[4];
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb)
+          asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+                       : "=r"(bh0[nb]), "=r"(bh1[nb]), "=r"(bm0[nb]), "=r"(bm1[nb])
+                       : "r"(vb + r * MT_COLS * 64 + (vl ^ (nb << 4))));
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Pm[r], bh0[nb], bh1[nb]);
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Ph[r], bm0[nb], bm1[nb]);
+#pragma unroll
+        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Ph[r], bh0[nb], bh1[nb]);
+      }
+      release();
+      const int qx = x0 + wx + g;
+      if (qx < W) {
+#pragma unroll
+        for (int half = 0; half < 2; ++half) {
+          const int qy = y0 + wy + half;
+          if (qy < H) {
+            float* o = out + ((size_t)(n * H + qy) * W + qx) * ldo + j * MCH + 2 * t;
+#pragma unroll
+            for (int nb = 0; nb < 4; ++nb)
+              *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
+          }
+        }
+      }
+    }
+  }
+}
+
+// 4-D tensor map {word, x, y, image} over the first 128 words of each pixel (row stride ld words), box of 16 words x
+// box_w x box_h pixels of one image, 64-byte swizzle, out-of-range pixels zero-filled
+bool window_map(CUtensorMap* m, const void* ptr, int ld, int N, int H, int W, int box_w, int box_h) {
+  tc::EncodeTiledFn enc = tc::get_encode();
+  if (!enc) return false;
+  const cuuint64_t row = 4ull * ld;
+  cuuint64_t dims[4] = {128, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
+  cuuint64_t strides[3] = {row, row * W, row * W * H};
+  cuuint32_t box[4] = {16, (cuuint32_t)box_w, (cuuint32_t)box_h, 1};
+  cuuint32_t estr[4] = {1, 1, 1, 1};
+  return enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT32, 4, const_cast<void*>(ptr), dims, strides, box, estr,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_64B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -856,11 +1046,11 @@ int di_lcab_window_pre_f32(const float* q, int ldq, const float* k, int ldk, con
   dim3 mgrid(di_cdiv(W, MQ_COLS), di_cdiv(H, MQ_ROWS), N);
   size_t smem = 2ull * BSTAGE_WORDS * sizeof(float);
   static DiSmemOnce once{};
-  if (!di_smem_once(once, lcab_window_pre_kernel<false>, (int)smem)) {
+  if (!di_smem_once(once, lcab_window_pre_kernel, (int)smem)) {
     di_set_error("di_lcab_window_pre_f32: cannot reserve shared memory");
     return DI_ERR_LAUNCH;
   }
-  lcab_window_pre_kernel<false><<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, 1.0f / sqrtf((float)C));
+  lcab_window_pre_kernel<<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, 1.0f / sqrtf((float)C));
   DI_CHECK_LAUNCH("di_lcab_window_pre_f32");
   return DI_OK;
 }
@@ -879,16 +1069,26 @@ int di_lcab_window_tc_f32(const void* q, int ldq, const void* k, int ldk, const 
                "di_lcab_window_tc_f32: strides must be multiples of 4 words and >= 128");
   DI_CHECK_ARG(((uintptr_t)q | (uintptr_t)k | (uintptr_t)v | (uintptr_t)out) % 16 == 0,
                "di_lcab_window_tc_f32: pointers must be 16-byte aligned");
-  dim3 mgrid(di_cdiv(W, MQ_COLS), di_cdiv(H, MQ_ROWS), N);
-  size_t smem = 2ull * BSTAGE_WORDS * sizeof(float);
+  const char* name = "di_lcab_window_tc_f32";
+  const long long tiles = (long long)N * di_cdiv(H, MQ_ROWS) * di_cdiv(W, MQ_COLS);
+  DI_CHECK_ARG(tiles < (1ll << 31), "%s: too many tiles", name);
+  int sms = 0;
+  const int rc = tc::sm_budget(name, &sms);
+  if (rc != DI_OK) return rc;
   static DiSmemOnce once{};
-  if (!di_smem_once(once, lcab_window_pre_kernel<true>, (int)smem)) {
-    di_set_error("di_lcab_window_tc_f32: cannot reserve shared memory");
+  if (!di_smem_once(once, lcab_window_tc_kernel, TC_SMEM_BYTES)) {
+    di_set_error("%s: cannot reserve %d bytes of shared memory", name, TC_SMEM_BYTES);
     return DI_ERR_LAUNCH;
   }
-  lcab_window_pre_kernel<true><<<mgrid, 256, smem, stream>>>(static_cast<const float*>(q), ldq, static_cast<const float*>(k), ldk,
-                                                             static_cast<const float*>(v), ldv, out, ldo, H, W, C,
-                                                             1.0f / sqrtf((float)C));
+  CUtensorMap maps[3];
+  if (!(window_map(&maps[0], q, ldq, N, H, W, MQ_COLS, MQ_ROWS) && window_map(&maps[1], k, ldk, N, H, W, MT_COLS, MT_ROWS) &&
+        window_map(&maps[2], v, ldv, N, H, W, MT_COLS, MT_ROWS))) {
+    di_set_error("%s: cuTensorMapEncodeTiled failed", name);
+    return DI_ERR_LAUNCH;
+  }
+  const int grid = tiles < sms ? (int)tiles : sms;
+  lcab_window_tc_kernel<<<grid, 256, TC_SMEM_BYTES, stream>>>(maps[0], maps[1], maps[2], out, ldo, H, W, di_cdiv(H, MQ_ROWS),
+                                                               di_cdiv(W, MQ_COLS), (int)tiles, 1.0f / sqrtf((float)C));
   DI_CHECK_LAUNCH("di_lcab_window_tc_f32");
   return DI_OK;
 }

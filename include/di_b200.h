@@ -110,7 +110,8 @@ int di_lcab_window_f32(const float* q, int ldq, const float* k, int ldk, const f
 int di_lcab_window_pre_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo,
                            int N, int H, int W, int C, cudaStream_t stream);
 
-/* The same op for PLANAR pre-split operands (split_kind 3 above; lcab.cu, bf16-split mma.sync tensor-core kernel):
+/* The same op for PLANAR pre-split operands (split_kind 3 above; lcab.cu, bf16-split mma.sync tensor-core kernel on a
+ * persistent grid of at most di_tc_set_sm_limit CTAs, operands loaded by TMA), bit-identical to di_lcab_window_pre_f32:
  * q, k, v -- [N*H*W] pixels with a stride of ld* 32-bit words, 128 bf16 hi | 128 bf16 mid per pixel;
  * out fp32 [N,H,W,ldo].  C must be 128 (returns -3 otherwise: use di_lcab_window_pre_f32 / di_lcab_window_f32).
  * Replaces similar_forward + softmax + weighting_forward (encoder_utils.py:132-134, localAttention.cpp:7-15,31-39). */

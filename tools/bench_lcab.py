@@ -7,6 +7,13 @@ Projection rates are quoted against the fused floor: each distinct input map rea
 4 F bytes for self attention and 5 F for cross attention (F = M * 128 * 4 bytes).  The peak is the H100 SXM data-sheet
 HBM3 bandwidth (3.35 TB/s) unless MEASURED_PEAKS.json gives a measured one.
 
+The window kernel's figures are computed from the shape and the kernel's tiling (8 x 16 queries per CTA, 8 warps of
+2 x 8 queries): its HBM floor (q, k, v read once and out written once, 512 bytes per pixel each), its mma.sync
+m16n8k16 count (per warp 4 chunks x 2 k16 steps x 20 key blocks x 3 split products for Q K^T plus 4 chunks x 10 halo
+rows x 4 channel blocks x 3 for P V) and the time that count takes at the data-sheet dense bf16 rate (989 TFLOP/s),
+its L2 -> shared-memory fill (per tile and 32-channel chunk: the 16 x 24 K halo and the 8 x 16 Q tile, then the V
+halo, 128 bytes per pixel), and the fraction of the HBM floor the measured time reaches.
+
     python tools/bench_lcab.py [--iters 20] [--only img|bev]      (needs an H100)
 """
 import argparse
@@ -35,6 +42,21 @@ def timed(fn, flush, iters):
         torch.cuda.synchronize()
         tot += a.elapsed_time(b)
     return tot / iters * 1e3
+
+
+BF16_TFLOPS = 989.0                                                # H100 SXM data sheet, dense
+
+
+def window_counts(N, H, W, peak_gbs):
+    """Shape-derived figures of the planar window kernel (C = 128)."""
+    M = N * H * W
+    tiles = N * -(-H // 8) * -(-W // 16)
+    floor = 4 * M * 512
+    mma = tiles * 8 * (4 * 2 * 20 * 3 + 4 * 10 * 4 * 3)
+    fill = tiles * 4 * ((16 * 24 + 8 * 16) + 16 * 24) * 128
+    return dict(tiles=tiles, hbm_floor_mb=round(floor / 1e6, 1), hbm_floor_us=round(floor / (peak_gbs * 1e9) * 1e6, 1),
+                mma_sync=mma, mma_us_at_datasheet=round(mma * 4096 / (BF16_TFLOPS * 1e12) * 1e6, 1),
+                l2_fill_mb=round(fill / 1e6, 1))
 
 
 def main():
@@ -83,6 +105,9 @@ def main():
         q, k, v = outs['fused']
         out = torch.empty(M, C, device=dev)
         res['window_us'] = round(timed(lambda: ops.lcab_window_tc(q, k, v, N, H, W, C, out=out), flush, args.iters), 1)
+        win = window_counts(N, H, W, peak)
+        win['frac_of_hbm_floor'] = round(win['hbm_floor_us'] / res['window_us'], 3)
+        res['window'] = win
         print(json.dumps(res), flush=True)
 
 
