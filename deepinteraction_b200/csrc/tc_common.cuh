@@ -52,6 +52,27 @@ __device__ __forceinline__ void tma_prefetch_2d(const CUtensorMap* map, int c0, 
                : "memory");
 }
 
+// TMA store of a shared-memory box (rows past the tensor's extent are not written), as one bulk group
+__device__ __forceinline__ void tma_store_2d(const CUtensorMap* map, uint32_t src, int c0, int c1) {
+  asm volatile("cp.async.bulk.tensor.2d.global.shared::cta.bulk_group [%0, {%2, %3}], [%1];" ::"l"(
+                   reinterpret_cast<uint64_t>(map)),
+               "r"(src), "r"(c0), "r"(c1)
+               : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the issuing thread's bulk groups have finished reading shared memory / have completed
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+// orders this thread's generic-proxy shared-memory writes before later async-proxy (TMA) accesses
+__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
+// named barriers (id 0 is __syncthreads); `threads` counts the participants of both bar_sync and bar_arrive
+__device__ __forceinline__ void bar_sync(int id, int threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+__device__ __forceinline__ void bar_arrive(int id, int threads) {
+  asm volatile("bar.arrive %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
+
 // wgmma shared-memory descriptor of a K-major, 128B-swizzled operand tile: rows of 128 bytes, 8-row atoms 1024 bytes
 // apart (SBO), tile 1024-byte aligned.  A k-step inside the 128-byte row is selected by adding its byte offset.
 __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {

@@ -131,6 +131,8 @@ int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, con
                      int M, cudaStream_t stream);
 /* 1 = the fused kernel (default), 0 = five separate bf16-split GEMM launches (process-wide; A/B runs and tests) */
 int di_lcab_proj_set_mode(int mode);
+/* CTAs per role (Q, K, V) the fused kernel launches for M rows under the current SM budget (di_tc_set_sm_limit) */
+int di_lcab_proj_grid(int M, int* nq, int* nk, int* nv);
 
 /* LocalContextAttentionBlock.forward for C = 128 as one call = di_lcab_proj_f32 + di_lcab_window_tc_f32 on `stream`
  * (models/utils/encoder_utils.py:119-135; SURVEY.md 8(b) `di_lcab_forward`).  qkv: workspace of 3 * N*H*W * 128 words. */

@@ -5,7 +5,8 @@ timed as separate calls with CUDA events, L2 flushed before every call.  Prints 
 
 Projection rates are quoted against the fused floor: each distinct input map read once and q, k, v written once,
 4 F bytes for self attention and 5 F for cross attention (F = M * 128 * 4 bytes).  The peak is the H100 SXM data-sheet
-HBM3 bandwidth (3.35 TB/s) unless MEASURED_PEAKS.json gives a measured one.
+HBM3 bandwidth (3.35 TB/s) unless MEASURED_PEAKS.json gives a measured one.  `proj_fused_ctas_qkv` is the number of
+Q, K and V CTAs the fused kernel launched.
 
 The window kernel's figures are computed from the shape and the kernel's tiling (8 x 16 queries per CTA, 8 warps of
 2 x 8 queries): its HBM floor (q, k, v read once and out written once, 512 bytes per pixel each), its mma.sync
@@ -17,6 +18,7 @@ halo, 128 bytes per pixel), and the fraction of the HBM floor the measured time 
     python tools/bench_lcab.py [--iters 20] [--only img|bev]      (needs an H100)
 """
 import argparse
+import ctypes
 import json
 import os
 import subprocess
@@ -64,7 +66,7 @@ def main():
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--only', default='')
     args = ap.parse_args()
-    from deepinteraction_b200 import mmri, ops, synth
+    from deepinteraction_b200 import _lib, mmri, ops, synth
     dev = torch.device('cuda:0')
     torch.set_grad_enabled(False)
     peak, peak_src = 3350.0, 'H100 SXM data sheet (3.35 TB/s)'
@@ -91,6 +93,9 @@ def main():
         floor = (4 if self_attn else 5) * F
         res = dict(shape=tag, M=M, gpu=gpu[0] if gpu else None, peak_gbs=peak, peak_source=peak_src,
                    proj_floor_mb=round(floor / 1e6, 1), proj_floor_us=round(floor / (peak * 1e9) * 1e6, 1))
+        roles = [ctypes.c_int() for _ in range(3)]
+        _lib.check(_lib.lib().di_lcab_proj_grid(M, *[ctypes.byref(r) for r in roles]), 'di_lcab_proj_grid')
+        res['proj_fused_ctas_qkv'] = [r.value for r in roles]
         outs = {}
         for arm, fused in (('fused', True), ('chain', False)):
             ops.set_lcab_fused(fused)
