@@ -43,7 +43,6 @@ SIGNATURES = {
     'di_lcab_window_pre_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p],
     'di_lcab_window_tc_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _p],
     'di_lcab_proj_f32': [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _p],
-    'di_lcab_proj_set_mode': [_i],
     'di_lcab_proj_grid': [_i, ctypes.POINTER(_i), ctypes.POINTER(_i), ctypes.POINTER(_i)],
     'di_lcab_forward_f32': [_p, _i, _p, _i, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _p],
     'di_set_window_ffma': [_i],

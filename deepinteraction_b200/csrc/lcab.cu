@@ -7,11 +7,16 @@
 // Semantics kept from the reference kernels: out-of-image taps have logit 0 and STILL take
 // softmax mass; their values are skipped.  Both fall out of zero-filling the halo.
 //
-// Layout: q/k/v/out are pixel-major (NHWC) fp32 with a per-pixel stride (ld*), so C channels of a
-// pixel are one contiguous 4*C-byte row.  One CTA = 16x16 queries; the (16+2r)^2 halo tile of k
-// (then v) streams through shared memory in 16-channel chunks with cp.async double buffering;
-// each thread keeps the k*k logits of its query in registers, so logits/probabilities never
-// touch HBM (the reference writes and re-reads 2*N*81*4 bytes per call).
+// Which kernel serves which path (q / k / v / out are pixel-major NHWC rows with a per-pixel stride):
+//   lcab_window_tc_kernel    planar bf16 hi | mid operands (di_lcab_window_tc_f32), C = 128: the product path, fed by
+//                            the fused projections of lcab_proj.cu (di_lcab_forward_f32).
+//   lcab_window_pre_kernel   interleaved pre-split operands (di_lcab_window_pre_f32) for the other C % 64 == 0, e.g.
+//                            C = 64, or C = 256 / 512 in config 5: the dense layers' epilogue writes them.
+//   lcab_window_bf16_kernel  fp32 operands split in shared memory (di_lcab_window_f32): the other C % 32 == 0, or when
+//                            the projections do not pre-split.
+//   lcab_window_kernel<KS>   FFMA (di_lcab_window_f32): ks = 3, or C % 32 != 0.
+// The three bf16-split kernels run one per-warp core (window_core below) and differ only in how the operands reach
+// shared memory and where a fragment lives there, so they are bit-identical on the same hi / mid words.
 #include "tc_common.cuh"
 
 namespace {
@@ -31,6 +36,11 @@ __device__ __forceinline__ void cp_async_wait() {
   asm volatile("cp.async.wait_group %0;\n" ::"n"(N));
 }
 
+// ------------------------------------------------------------------------------------------------
+// FFMA kernel.  One CTA = 16x16 queries; the (16+2r)^2 halo tile of k (then v) streams through shared memory in
+// 16-channel chunks with cp.async double buffering; each thread keeps the k*k logits of its query in registers, so
+// logits/probabilities never touch HBM (the reference writes and re-reads 2*N*81*4 bytes per call).
+// ------------------------------------------------------------------------------------------------
 template <int KS>
 __global__ void __launch_bounds__(TQ * TQ, 1)
 lcab_window_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
@@ -148,220 +158,30 @@ lcab_window_kernel(const float* __restrict__ q, int ldq, const float* __restrict
   }
 }
 
-
 // ------------------------------------------------------------------------------------------------
-// Tensor-core version of the 9x9 window attention (the one the product path launches).
-// One CTA = 8 query rows x 16 query columns; a warp owns a 2 x 8 patch of queries (M = 16).  Both contractions run
-// on mma.sync.m16n8k8 TF32 with error compensation (hi/lo split of both operands, 3 products), so logits and
-// outputs stay fp32-faithful:
-//   S[16 x (10 rows x 16 cols)] = Q K^T  -> 20 key blocks of 8; accumulated over 32-channel chunks
+// window_core: the per-warp math of the three bf16-split tensor-core kernels.
+// One CTA = 8 query rows x 16 query columns; a warp owns a 2 x 8 patch of queries (M = 16) at (wy, wx) of the tile.
+// Every operand x is split into hi = bf16(x), mid = bf16(x - hi) (16 mantissa bits kept, product error ~1e-5), and each
+// contraction runs on mma.sync.m16n8k16 bf16 as the three products mid.hi, hi.mid, hi.hi:
+//   S[16 x (10 rows x 16 cols)] = Q K^T  -> 20 key blocks of 8 (block b = halo row b / 2, column block b % 2),
+//                                           accumulated over 32-channel chunks in k16 steps
 //   softmax over the 81 in-window keys of each query, entirely in registers (quad shuffles)
-//   O[16 x C] = P V                       -> the S accumulator fragments are re-used as the A operand by pairing
-//                                            k-index t <-> key 2t and t+4 <-> key 2t+1 of each block
+//   O[16 x C] = P V                       -> the S accumulator fragments are re-used as the A operand: for halo row r,
+//                                            k16 = the 16 halo columns wx .. wx+15
 // Band structure: a query uses 9 of the 16 key columns and 9 of the 10 key rows of its patch (1.98x padding).
-// The key/value halo tile (16 x 24 pixels x 32 channels) and the query tile stream through shared memory with
-// cp.async double buffering; zero-filled halo pixels give the reference's out-of-image rule (logit 0 kept in the
-// softmax, value skipped).
+// The issue order of the mma.sync below is part of the result: per accumulator it fixes the summation order (so the
+// bits), and product-major order across accumulators keeps consecutive mma.sync off one accumulator (the legacy
+// tensor path has a long issue-to-result latency; 3 back-to-back products into one fragment serialise on it).
 // ------------------------------------------------------------------------------------------------
-constexpr int MQ_ROWS = 8, MQ_COLS = 16, MCH = 32, MSTR = MCH + 4;   // padded pixel stride: conflict-free fragments
-constexpr int MT_ROWS = MQ_ROWS + 8, MT_COLS = MQ_COLS + 8;
-constexpr int MKV_FLOATS = MT_ROWS * MT_COLS * MSTR;                  // 13824
-constexpr int MQ_FLOATS = MQ_ROWS * MQ_COLS * MSTR;                   // 4608
-constexpr int MSTAGE_FLOATS = MKV_FLOATS + MQ_FLOATS;
-
-__device__ __forceinline__ void mma_tf32(float (&c)[4], const uint32_t (&a)[4], uint32_t b0, uint32_t b1) {
-  asm volatile(
-      "mma.sync.aligned.m16n8k8.row.col.f32.tf32.tf32.f32 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
-      : "+f"(c[0]), "+f"(c[1]), "+f"(c[2]), "+f"(c[3])
-      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
-}
-__device__ __forceinline__ void split_tf32(float x, uint32_t& hi, uint32_t& lo) {
-  hi = __float_as_uint(x) & 0xFFFFE000u;
-  lo = __float_as_uint(x - __uint_as_float(hi));
-}
-
-__global__ void __launch_bounds__(256, 1)
-lcab_window_mma_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
-                       const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
-                       float scale) {
-  extern __shared__ __align__(16) float smem[];   // [2][MKV_FLOATS + MQ_FLOATS]
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int x0 = blockIdx.x * MQ_COLS, y0 = blockIdx.y * MQ_ROWS, n = blockIdx.z;
-  const size_t img_off = (size_t)n * H * W;
-  const int nchunk = C / MCH;
-  const int nstage = 2 * nchunk;
-
-  auto issue = [&](int stage) {
-    const bool is_k = stage < nchunk;
-    const float* src = is_k ? k : v;
-    const int ld = is_k ? ldk : ldv;
-    const int c0 = (is_k ? stage : stage - nchunk) * MCH;
-    float* dst = smem + (stage & 1) * MSTAGE_FLOATS;
-    for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
-      int px = i / (MCH / 4), c4 = i % (MCH / 4);
-      int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
-      bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
-      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
-      cp_async16(dst + px * MSTR + c4 * 4, gp, ok);
-    }
-    if (is_k) {
-      float* qd = dst + MKV_FLOATS;
-      for (int i = tid; i < MQ_ROWS * MQ_COLS * (MCH / 4); i += 256) {
-        int px = i / (MCH / 4), c4 = i % (MCH / 4);
-        int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
-        bool ok = gy < H && gx < W;
-        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
-        cp_async16(qd + px * MSTR + c4 * 4, gp, ok);
-      }
-    }
-    cp_async_commit();
-  };
-
-  // warp -> 2 query rows x 8 query columns (M = 16): fragment rows g = (row wy, col wx+g), g+8 = (row wy+1, col wx+g).
-  // Keys: 10 halo rows (wy .. wy+9 in tile coordinates) x 16 halo columns (wx .. wx+15) = 20 blocks of 8.
-  const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
-  float S[20][4];
-#pragma unroll
-  for (int b = 0; b < 20; ++b) S[b][0] = S[b][1] = S[b][2] = S[b][3] = 0.f;
-
-  issue(0);
-  for (int stage = 0; stage < nstage; ++stage) {
-    if (stage + 1 < nstage) {
-      issue(stage + 1);
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    const float* kv = smem + (stage & 1) * MSTAGE_FLOATS;
-    if (stage < nchunk) {
-      // ---------------- S += Q[chunk] K[chunk]^T ----------------
-      const float* qs = kv + MKV_FLOATS + (wy * MQ_COLS + wx) * MSTR;
-#pragma unroll
-      for (int ks = 0; ks < MCH / 8; ++ks) {
-        uint32_t ah[4], al[4];
-        split_tf32(qs[g * MSTR + ks * 8 + t], ah[0], al[0]);
-        split_tf32(qs[(MQ_COLS + g) * MSTR + ks * 8 + t], ah[1], al[1]);
-        split_tf32(qs[g * MSTR + ks * 8 + t + 4], ah[2], al[2]);
-        split_tf32(qs[(MQ_COLS + g) * MSTR + ks * 8 + t + 4], ah[3], al[3]);
-#pragma unroll
-        for (int r = 0; r < 10; ++r)
-#pragma unroll
-          for (int cb = 0; cb < 2; ++cb) {
-            const float* kp = kv + ((wy + r) * MT_COLS + wx + cb * 8 + g) * MSTR + ks * 8 + t;
-            uint32_t bh0, bl0, bh1, bl1;
-            split_tf32(kp[0], bh0, bl0);
-            split_tf32(kp[4], bh1, bl1);
-            mma_tf32(S[r * 2 + cb], al, bh0, bh1);
-            mma_tf32(S[r * 2 + cb], ah, bl0, bl1);
-            mma_tf32(S[r * 2 + cb], ah, bh0, bh1);
-          }
-      }
-      if (stage == nchunk - 1) {
-        // ---------------- masked softmax over the 81 in-window keys ----------------
-        float m0 = -INFINITY, m1 = -INFINITY;   // fragment rows g (query row wy) and g+8 (query row wy+1)
-#pragma unroll
-        for (int b = 0; b < 20; ++b) {
-          const int r = b >> 1, cb = b & 1;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int d = cb * 8 + 2 * t + j - g;               // key column - query column + 4
-            const bool colok = d >= 0 && d <= 8;
-            S[b][j] = (colok && r <= 8) ? S[b][j] * scale : -INFINITY;
-            S[b][2 + j] = (colok && r >= 1) ? S[b][2 + j] * scale : -INFINITY;
-            m0 = fmaxf(m0, S[b][j]);
-            m1 = fmaxf(m1, S[b][2 + j]);
-          }
-        }
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int b = 0; b < 20; ++b)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            S[b][j] = expf(S[b][j] - m0);            // exp(-inf) = 0 for out-of-window entries
-            S[b][2 + j] = expf(S[b][2 + j] - m1);
-            s0 += S[b][j];
-            s1 += S[b][2 + j];
-          }
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        const float i0 = 1.f / s0, i1 = 1.f / s1;
-#pragma unroll
-        for (int b = 0; b < 20; ++b) {
-          S[b][0] *= i0; S[b][1] *= i0; S[b][2] *= i1; S[b][3] *= i1;
-        }
-      }
-    } else {
-      // ---------------- O[chunk] = P V[chunk] ----------------
-      float O[MCH / 8][4];
-#pragma unroll
-      for (int nb = 0; nb < MCH / 8; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
-#pragma unroll
-      for (int r = 0; r < 10; ++r)
-#pragma unroll
-        for (int cb = 0; cb < 2; ++cb) {
-          const int b = r * 2 + cb;
-          uint32_t ah[4], al[4];                       // A = P block with k-index t <-> key 2t, t+4 <-> key 2t+1
-          split_tf32(S[b][0], ah[0], al[0]);
-          split_tf32(S[b][2], ah[1], al[1]);
-          split_tf32(S[b][1], ah[2], al[2]);
-          split_tf32(S[b][3], ah[3], al[3]);
-          const float* vp = kv + ((wy + r) * MT_COLS + wx + cb * 8 + 2 * t) * MSTR + g;
-#pragma unroll
-          for (int nb = 0; nb < MCH / 8; ++nb) {
-            uint32_t bh0, bl0, bh1, bl1;
-            split_tf32(vp[nb * 8], bh0, bl0);
-            split_tf32(vp[MSTR + nb * 8], bh1, bl1);
-            mma_tf32(O[nb], al, bh0, bh1);
-            mma_tf32(O[nb], ah, bl0, bl1);
-            mma_tf32(O[nb], ah, bh0, bh1);
-          }
-        }
-      const int cbase = (stage - nchunk) * MCH;
-      const int qx = x0 + wx + g;
-      if (qx < W) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int qy = y0 + wy + half;
-          if (qy < H) {
-            float* o = out + (img_off + (size_t)qy * W + qx) * ldo + cbase + 2 * t;
-#pragma unroll
-            for (int nb = 0; nb < MCH / 8; ++nb)
-              *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
-          }
-        }
-      }
-    }
-    __syncthreads();
-  }
-}
-
-// ------------------------------------------------------------------------------------------------
-// bf16-split version of the kernel above (the default): same tiling, same fragment algebra, but every operand is
-// split ONCE per shared-memory stage into hi = bf16(x), mid = bf16(x - hi) (16 mantissa bits kept, product error
-// ~1e-5) instead of per fragment load, and the contractions run on mma.sync.m16n8k16 bf16 (3 products per k16
-// instead of 3 per k8: half the tensor instructions, ~1/4 of the splitting arithmetic).
-//   K / Q chunk: cp.async lands fp32 [pixel][32 ch]; a conversion pass rewrites each channel pair IN PLACE as the
-//                64-bit word (hi bf16x2, mid bf16x2)  -> B / A fragments are single LDS.64, conflict-free with a
-//                pixel stride of 40 words
-//   V chunk:     the k index of P V is the key, so V is re-laid as [key pair along x][channel] -> (hi, mid) words in
-//                a separate buffer (pair stride 72 words)
-//   P:           after the softmax the 20 S accumulator fragments ARE the A fragments of P V (k16 = the 16 halo
-//                columns of one halo row); they are packed to hi / mid once and reused for every V chunk
-// ------------------------------------------------------------------------------------------------
-constexpr int BSTR = 40;                                             // words per pixel of the K / Q landing rows
+constexpr int MQ_ROWS = 8, MQ_COLS = 16, MCH = 32;                  // query tile, channels per chunk
+constexpr int MT_ROWS = MQ_ROWS + 8, MT_COLS = MQ_COLS + 8;          // key / value halo tile
+constexpr int BSTR = 40;                                             // words per pixel of the interleaved K / Q rows
 constexpr int BKV_WORDS = MT_ROWS * MT_COLS * BSTR;                  // 15360
 constexpr int BQ_WORDS = MQ_ROWS * MQ_COLS * BSTR;                   // 5120
 constexpr int BSTAGE_WORDS = BKV_WORDS + BQ_WORDS;                   // 20480 (80 KB)
 constexpr int VPSTR = 72;                                            // words per key pair of the packed V chunk
 constexpr int VPK_WORDS = MT_ROWS * (MT_COLS / 2) * VPSTR;           // 13824 (54 KB)
+constexpr int VSTR2 = 36;                                            // pre-split V pixel stride: 8 ldmatrix rows -> 32 banks
 
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
   uint32_t r;
@@ -380,203 +200,30 @@ __device__ __forceinline__ void mma_bf16(float (&c)[4], const uint32_t (&a)[4], 
       : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "r"(b0), "r"(b1));
 }
 
-__global__ void __launch_bounds__(256, 1)
-lcab_window_bf16_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
-                        const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
-                        float scale) {
-  extern __shared__ __align__(16) float smem[];   // [2][BSTAGE_WORDS] landing / converted K,Q | [VPK_WORDS] packed V
-  uint32_t* vpk = reinterpret_cast<uint32_t*>(smem + 2 * BSTAGE_WORDS);
-  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  const int g = lane >> 2, t = lane & 3;
-  const int x0 = blockIdx.x * MQ_COLS, y0 = blockIdx.y * MQ_ROWS, n = blockIdx.z;
-  const size_t img_off = (size_t)n * H * W;
-  const int nchunk = C / MCH;
-  const int nstage = 2 * nchunk;
-
-  auto issue = [&](int stage) {
-    const bool is_k = stage < nchunk;
-    const float* src = is_k ? k : v;
-    const int ld = is_k ? ldk : ldv;
-    const int c0 = (is_k ? stage : stage - nchunk) * MCH;
-    float* dst = smem + (stage & 1) * BSTAGE_WORDS;
-    for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
-      int px = i / (MCH / 4), c4 = i % (MCH / 4);
-      int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
-      bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
-      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
-      cp_async16(dst + px * BSTR + c4 * 4, gp, ok);
-    }
-    if (is_k) {
-      float* qd = dst + BKV_WORDS;
-      for (int i = tid; i < MQ_ROWS * MQ_COLS * (MCH / 4); i += 256) {
-        int px = i / (MCH / 4), c4 = i % (MCH / 4);
-        int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
-        bool ok = gy < H && gx < W;
-        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
-        cp_async16(qd + px * BSTR + c4 * 4, gp, ok);
-      }
-    }
-    cp_async_commit();
-  };
-
-  const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
-  float S[20][4];
+template <int N>
+__device__ __forceinline__ void zero_acc(float (&acc)[N][4]) {
 #pragma unroll
-  for (int b = 0; b < 20; ++b) S[b][0] = S[b][1] = S[b][2] = S[b][3] = 0.f;
-  uint32_t Ph[10][4], Pm[10][4];                     // P = softmax(S) as packed bf16 hi / mid A fragments
-
-  issue(0);
-  for (int stage = 0; stage < nstage; ++stage) {
-    if (stage + 1 < nstage) {
-      issue(stage + 1);
-      cp_async_wait<1>();
-    } else {
-      cp_async_wait<0>();
-    }
-    __syncthreads();
-    float* buf = smem + (stage & 1) * BSTAGE_WORDS;
-    if (stage < nchunk) {
-      // ---- split K and Q in place: channel pair (2j, 2j+1) of a pixel -> (hi, mid) ----
-      for (int i = tid; i < (MT_ROWS * MT_COLS + MQ_ROWS * MQ_COLS) * (MCH / 2); i += 256) {
-        float* pp = buf + (i >> 4) * BSTR + (i & 15) * 2;
-        const float2 x = *reinterpret_cast<const float2*>(pp);
-        *reinterpret_cast<uint2*>(pp) = split_bf16x2(x.x, x.y);
-      }
-      __syncthreads();
-      // ---------------- S += Q[chunk] K[chunk]^T ----------------
-      const uint32_t* kw = reinterpret_cast<const uint32_t*>(buf);
-      const uint32_t* qw = kw + BKV_WORDS + (wy * MQ_COLS + wx) * BSTR;
-#pragma unroll
-      for (int ks = 0; ks < MCH / 16; ++ks) {
-        uint32_t ah[4], am[4];
-        {
-          const uint2 a0 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t) * 2);
-          const uint2 a1 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t) * 2);
-          const uint2 a2 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t + 4) * 2);
-          const uint2 a3 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t + 4) * 2);
-          ah[0] = a0.x; am[0] = a0.y; ah[1] = a1.x; am[1] = a1.y;
-          ah[2] = a2.x; am[2] = a2.y; ah[3] = a3.x; am[3] = a3.y;
-        }
-        // 4 key blocks at a time, product-major: consecutive mma.sync never share an accumulator (the legacy
-        // tensor path has a long issue-to-result latency; 3 back-to-back products into one fragment serialise on it)
-#pragma unroll
-        for (int r2 = 0; r2 < 5; ++r2) {
-          uint2 b0[4], b1[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const uint32_t* kp = kw + ((wy + 2 * r2 + (u >> 1)) * MT_COLS + wx + (u & 1) * 8 + g) * BSTR + (ks * 8 + t) * 2;
-            b0[u] = *reinterpret_cast<const uint2*>(kp);
-            b1[u] = *reinterpret_cast<const uint2*>(kp + 8);
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].y, b1[u].y);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
-        }
-      }
-      if (stage == nchunk - 1) {
-        // ---------------- masked softmax over the 81 in-window keys ----------------
-        float m0 = -INFINITY, m1 = -INFINITY;   // fragment rows g (query row wy) and g+8 (query row wy+1)
-#pragma unroll
-        for (int b = 0; b < 20; ++b) {
-          const int r = b >> 1, cb = b & 1;
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            const int d = cb * 8 + 2 * t + j - g;               // key column - query column + 4
-            const bool colok = d >= 0 && d <= 8;
-            S[b][j] = (colok && r <= 8) ? S[b][j] * scale : -INFINITY;
-            S[b][2 + j] = (colok && r >= 1) ? S[b][2 + j] * scale : -INFINITY;
-            m0 = fmaxf(m0, S[b][j]);
-            m1 = fmaxf(m1, S[b][2 + j]);
-          }
-        }
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 1));
-        m0 = fmaxf(m0, __shfl_xor_sync(0xffffffffu, m0, 2));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 1));
-        m1 = fmaxf(m1, __shfl_xor_sync(0xffffffffu, m1, 2));
-        float s0 = 0.f, s1 = 0.f;
-#pragma unroll
-        for (int b = 0; b < 20; ++b)
-#pragma unroll
-          for (int j = 0; j < 2; ++j) {
-            S[b][j] = expf(S[b][j] - m0);            // exp(-inf) = 0 for out-of-window entries
-            S[b][2 + j] = expf(S[b][2 + j] - m1);
-            s0 += S[b][j];
-            s1 += S[b][2 + j];
-          }
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 1);
-        s0 += __shfl_xor_sync(0xffffffffu, s0, 2);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 1);
-        s1 += __shfl_xor_sync(0xffffffffu, s1, 2);
-        const float i0 = 1.f / s0, i1 = 1.f / s1;
-        // A fragments of P V for halo row r: k = the 16 halo columns wx .. wx+15 (block cb=0 -> k 0..7, cb=1 -> 8..15)
-#pragma unroll
-        for (int r = 0; r < 10; ++r)
-#pragma unroll
-          for (int cb = 0; cb < 2; ++cb) {
-            const uint2 lo = split_bf16x2(S[r * 2 + cb][0] * i0, S[r * 2 + cb][1] * i0);   // row g
-            const uint2 hi = split_bf16x2(S[r * 2 + cb][2] * i1, S[r * 2 + cb][3] * i1);   // row g + 8
-            Ph[r][cb * 2] = lo.x; Pm[r][cb * 2] = lo.y;
-            Ph[r][cb * 2 + 1] = hi.x; Pm[r][cb * 2 + 1] = hi.y;
-          }
-      }
-    } else {
-      // ---- re-lay the V chunk: (key 2i, key 2i+1 of a halo row) x channel -> (hi, mid) ----
-      for (int i = tid; i < MT_ROWS * (MT_COLS / 2) * MCH; i += 256) {
-        const int c = i & (MCH - 1), pr = i >> 5;               // pr = row * 12 + pair
-        const int px = (pr / (MT_COLS / 2)) * MT_COLS + (pr % (MT_COLS / 2)) * 2;
-        const float v0 = buf[px * BSTR + c], v1 = buf[(px + 1) * BSTR + c];
-        *reinterpret_cast<uint2*>(vpk + pr * VPSTR + 2 * c) = split_bf16x2(v0, v1);
-      }
-      __syncthreads();
-      // ---------------- O[chunk] = P V[chunk] ----------------
-      float O[MCH / 8][4];
-#pragma unroll
-      for (int nb = 0; nb < MCH / 8; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
-#pragma unroll
-      for (int r = 0; r < 10; ++r) {
-        const uint32_t* vp = vpk + ((wy + r) * (MT_COLS / 2) + wx / 2 + t) * VPSTR + 2 * g;
-        uint2 b0[MCH / 8], b1[MCH / 8];
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) {
-          b0[nb] = *reinterpret_cast<const uint2*>(vp + nb * 16);
-          b1[nb] = *reinterpret_cast<const uint2*>(vp + 4 * VPSTR + nb * 16);
-        }
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Pm[r], b0[nb].x, b1[nb].x);
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph[r], b0[nb].y, b1[nb].y);
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph[r], b0[nb].x, b1[nb].x);
-      }
-      const int cbase = (stage - nchunk) * MCH;
-      const int qx = x0 + wx + g;
-      if (qx < W) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int qy = y0 + wy + half;
-          if (qy < H) {
-            float* o = out + (img_off + (size_t)qy * W + qx) * ldo + cbase + 2 * t;
-#pragma unroll
-            for (int nb = 0; nb < MCH / 8; ++nb)
-              *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
-          }
-        }
-      }
-    }
-    __syncthreads();
-  }
+  for (int b = 0; b < N; ++b) acc[b][0] = acc[b][1] = acc[b][2] = acc[b][3] = 0.f;
 }
 
-// ------------------------------------------------------------------------------------------------
-// Same kernel for PRE-SPLIT operands: q, k (kind 1) and v (kind 2) were written by the producing dense layer's
-// epilogue already as bf16 (hi, mid) words (gemm_tc.cu), 4 bytes per value at the value's own position.
-// The two conversion passes, one barrier per stage and the packed-V buffer disappear: stages go straight from
-// cp.async to fragments (LDS.64 for Q/K, ldmatrix.x4.trans for V).
-// ------------------------------------------------------------------------------------------------
-constexpr int VSTR2 = 36;                                            // V chunk pixel stride: 8 ldmatrix rows -> 32 distinct banks
+// S += Q K^T for one k16 step.  ah / am: the Q A fragment (hi, mid).  kfrag(b, b0, b1) loads the B fragment of key
+// block b: b0 = its first k half (k = t, hi in .x, mid in .y), b1 = its second (k = t + 4).
+template <class KFrag>
+__device__ __forceinline__ void qk_step(float (&S)[20][4], const uint32_t (&ah)[4], const uint32_t (&am)[4], KFrag kfrag) {
+  // 4 key blocks at a time, product-major
+#pragma unroll
+  for (int r2 = 0; r2 < 5; ++r2) {
+    uint2 b0[4], b1[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) kfrag(r2 * 4 + u, b0[u], b1[u]);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].y, b1[u].y);
+#pragma unroll
+    for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
+  }
+}
 
 // Masked softmax over the 81 in-window keys of the warp's two query rows (fragment rows g: query row wy, g + 8: row
 // wy + 1), then P = softmax(S) packed as the bf16 hi / mid A fragments of P V: for halo row r, k = the 16 halo columns
@@ -627,49 +274,120 @@ __device__ __forceinline__ void window_softmax(float (&S)[20][4], float scale, i
     }
 }
 
+// O += P V for one halo row (k16 = its 16 keys).  b0[nb] / b1[nb]: the B fragment of channel block nb for keys 0-7 /
+// 8-15, hi in .x, mid in .y.
+__device__ __forceinline__ void pv_row(float (&O)[MCH / 8][4], const uint32_t (&Ph)[4], const uint32_t (&Pm)[4],
+                                       const uint2 (&b0)[MCH / 8], const uint2 (&b1)[MCH / 8]) {
+#pragma unroll
+  for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Pm, b0[nb].x, b1[nb].x);
+#pragma unroll
+  for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph, b0[nb].y, b1[nb].y);
+#pragma unroll
+  for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph, b0[nb].x, b1[nb].x);
+}
+
+// V B fragments of one halo row by ldmatrix.x4.trans: the lane's row address picks keys 0-7 / 8-15 (matrices 0 / 1,
+// hi) and their mid parts (matrices 2 / 3), so the [key][channel] rows arrive as (k = key pair, n = channel) fragments.
+__device__ __forceinline__ void ldsm_v(uint32_t addr, uint2& b0, uint2& b1) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(b0.x), "=r"(b1.x), "=r"(b0.y), "=r"(b1.y)
+               : "r"(addr));
+}
+
+// out = the warp's 2 x 8 patch of one 32-channel chunk: query (qy0 + half, qx) of image n, channels c + nb * 8 + 2t
+__device__ __forceinline__ void store_patch(const float (&O)[MCH / 8][4], float* __restrict__ out, int ldo,
+                                            int n, int H, int W, int qy0, int qx, int c, int t) {
+  if (qx < W) {
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      const int qy = qy0 + half;
+      if (qy < H) {
+        float* o = out + ((size_t)(n * H + qy) * W + qx) * ldo + c + 2 * t;
+#pragma unroll
+        for (int nb = 0; nb < MCH / 8; ++nb)
+          *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
+      }
+    }
+  }
+}
+
+// S += Q K^T over one 32-channel chunk held as interleaved (hi, mid) words, pixel stride BSTR: kw = the 16 x 24 K halo,
+// qw = the warp's first query pixel in the 8 x 16 Q tile
+__device__ __forceinline__ void qk_chunk_interleaved(float (&S)[20][4], const uint32_t* kw, const uint32_t* qw, int wy,
+                                                     int wx, int g, int t) {
+#pragma unroll
+  for (int ks = 0; ks < MCH / 16; ++ks) {
+    uint32_t ah[4], am[4];
+    {
+      const uint2 a0 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t) * 2);
+      const uint2 a1 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t) * 2);
+      const uint2 a2 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t + 4) * 2);
+      const uint2 a3 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t + 4) * 2);
+      ah[0] = a0.x; am[0] = a0.y; ah[1] = a1.x; am[1] = a1.y;
+      ah[2] = a2.x; am[2] = a2.y; ah[3] = a3.x; am[3] = a3.y;
+    }
+    qk_step(S, ah, am, [&](int b, uint2& b0, uint2& b1) {
+      const uint32_t* kp = kw + ((wy + (b >> 1)) * MT_COLS + wx + (b & 1) * 8 + g) * BSTR + (ks * 8 + t) * 2;
+      b0 = *reinterpret_cast<const uint2*>(kp);
+      b1 = *reinterpret_cast<const uint2*>(kp + 8);
+    });
+  }
+}
+
+// cp.async of one 32-channel chunk of src (K or V) over the 16 x 24 halo tile (pixel stride pstr words, zero fill
+// outside the image) and, with a q, of the 8 x 16 Q tile (pixel stride BSTR), into dst; commits one group
+__device__ __forceinline__ void stage_chunk(float* dst, const float* __restrict__ src, int ld, int pstr,
+                                            const float* __restrict__ q, int ldq, int c0, size_t img_off, int x0, int y0,
+                                            int H, int W, int tid) {
+  for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
+    int px = i / (MCH / 4), c4 = i % (MCH / 4);
+    int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
+    bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
+    const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
+    cp_async16(dst + px * pstr + c4 * 4, gp, ok);
+  }
+  if (q) {
+    float* qd = dst + BKV_WORDS;
+    for (int i = tid; i < MQ_ROWS * MQ_COLS * (MCH / 4); i += 256) {
+      int px = i / (MCH / 4), c4 = i % (MCH / 4);
+      int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
+      bool ok = gy < H && gx < W;
+      const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
+      cp_async16(qd + px * BSTR + c4 * 4, gp, ok);
+    }
+  }
+  cp_async_commit();
+}
+
+// ------------------------------------------------------------------------------------------------
+// fp32 operands (di_lcab_window_f32).  cp.async lands each chunk as fp32 and the CTA splits it in shared memory, once
+// per stage rather than per fragment load:
+//   K / Q chunk: [pixel][32 ch] rewritten IN PLACE, channel pair (2j, 2j+1) -> the 64-bit word (hi bf16x2, mid
+//                bf16x2), the interleaved layout the dense layers' split epilogue writes (kind 1)
+//   V chunk:     the k index of P V is the key, so V is re-laid as [key pair along x][channel] -> (hi, mid) words in
+//                a separate buffer (pair stride 72 words)
+// ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(256, 1)
-lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
-                       const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
-                       float scale) {
-  extern __shared__ __align__(16) float smem[];   // [2][BSTAGE_WORDS]: K,Q chunk (pixel stride 40 words) or V chunk (36)
+lcab_window_bf16_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
+                        const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
+                        float scale) {
+  extern __shared__ __align__(16) float smem[];   // [2][BSTAGE_WORDS] landing / converted K,Q | [VPK_WORDS] packed V
+  uint32_t* vpk = reinterpret_cast<uint32_t*>(smem + 2 * BSTAGE_WORDS);
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int g = lane >> 2, t = lane & 3;
   const int x0 = blockIdx.x * MQ_COLS, y0 = blockIdx.y * MQ_ROWS, n = blockIdx.z;
   const size_t img_off = (size_t)n * H * W;
   const int nchunk = C / MCH;
   const int nstage = 2 * nchunk;
-
   auto issue = [&](int stage) {
     const bool is_k = stage < nchunk;
-    const float* src = is_k ? k : v;
-    const int ld = is_k ? ldk : ldv;
-    const int c0 = (is_k ? stage : stage - nchunk) * MCH;
-    float* dst = smem + (stage & 1) * BSTAGE_WORDS;
-    const int pstr = is_k ? BSTR : VSTR2;
-    for (int i = tid; i < MT_ROWS * MT_COLS * (MCH / 4); i += 256) {
-      int px = i / (MCH / 4), c4 = i % (MCH / 4);
-      int gy = y0 - 4 + px / MT_COLS, gx = x0 - 4 + px % MT_COLS;
-      bool ok = gy >= 0 && gy < H && gx >= 0 && gx < W;
-      const float* gp = ok ? src + (img_off + (size_t)gy * W + gx) * ld + c0 + c4 * 4 : src;
-      cp_async16(dst + px * pstr + c4 * 4, gp, ok);
-    }
-    if (is_k) {
-      float* qd = dst + BKV_WORDS;
-      for (int i = tid; i < MQ_ROWS * MQ_COLS * (MCH / 4); i += 256) {
-        int px = i / (MCH / 4), c4 = i % (MCH / 4);
-        int gy = y0 + px / MQ_COLS, gx = x0 + px % MQ_COLS;
-        bool ok = gy < H && gx < W;
-        const float* gp = ok ? q + (img_off + (size_t)gy * W + gx) * ldq + c0 + c4 * 4 : q;
-        cp_async16(qd + px * BSTR + c4 * 4, gp, ok);
-      }
-    }
-    cp_async_commit();
+    stage_chunk(smem + (stage & 1) * BSTAGE_WORDS, is_k ? k : v, is_k ? ldk : ldv, BSTR, is_k ? q : nullptr, ldq,
+                (is_k ? stage : stage - nchunk) * MCH, img_off, x0, y0, H, W, tid);
   };
 
   const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
   float S[20][4];
-#pragma unroll
-  for (int b = 0; b < 20; ++b) S[b][0] = S[b][1] = S[b][2] = S[b][3] = 0.f;
+  zero_acc(S);
   uint32_t Ph[10][4], Pm[10][4];                     // P = softmax(S) as packed bf16 hi / mid A fragments
 
   issue(0);
@@ -683,88 +401,107 @@ lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __rest
     __syncthreads();
     float* buf = smem + (stage & 1) * BSTAGE_WORDS;
     if (stage < nchunk) {
-      // ---------------- S += Q[chunk] K[chunk]^T ----------------
-      const uint32_t* kw = reinterpret_cast<const uint32_t*>(buf);
-      const uint32_t* qw = kw + BKV_WORDS + (wy * MQ_COLS + wx) * BSTR;
-#pragma unroll
-      for (int ks = 0; ks < MCH / 16; ++ks) {
-        uint32_t ah[4], am[4];
-        {
-          const uint2 a0 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t) * 2);
-          const uint2 a1 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t) * 2);
-          const uint2 a2 = *reinterpret_cast<const uint2*>(qw + g * BSTR + (ks * 8 + t + 4) * 2);
-          const uint2 a3 = *reinterpret_cast<const uint2*>(qw + (MQ_COLS + g) * BSTR + (ks * 8 + t + 4) * 2);
-          ah[0] = a0.x; am[0] = a0.y; ah[1] = a1.x; am[1] = a1.y;
-          ah[2] = a2.x; am[2] = a2.y; ah[3] = a3.x; am[3] = a3.y;
-        }
-        // 4 key blocks at a time, product-major: consecutive mma.sync never share an accumulator (the legacy
-        // tensor path has a long issue-to-result latency; 3 back-to-back products into one fragment serialise on it)
-#pragma unroll
-        for (int r2 = 0; r2 < 5; ++r2) {
-          uint2 b0[4], b1[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const uint32_t* kp = kw + ((wy + 2 * r2 + (u >> 1)) * MT_COLS + wx + (u & 1) * 8 + g) * BSTR;
-            b0[u] = *reinterpret_cast<const uint2*>(kp + 2 * (ks * 8 + t));
-            b1[u] = *reinterpret_cast<const uint2*>(kp + 2 * (ks * 8 + t + 4));
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].y, b1[u].y);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
-        }
+      // ---- split K and Q in place: channel pair (2j, 2j+1) of a pixel -> (hi, mid) ----
+      for (int i = tid; i < (MT_ROWS * MT_COLS + MQ_ROWS * MQ_COLS) * (MCH / 2); i += 256) {
+        float* pp = buf + (i >> 4) * BSTR + (i & 15) * 2;
+        const float2 x = *reinterpret_cast<const float2*>(pp);
+        *reinterpret_cast<uint2*>(pp) = split_bf16x2(x.x, x.y);
       }
+      __syncthreads();
+      const uint32_t* kw = reinterpret_cast<const uint32_t*>(buf);
+      qk_chunk_interleaved(S, kw, kw + BKV_WORDS + (wy * MQ_COLS + wx) * BSTR, wy, wx, g, t);
       if (stage == nchunk - 1) window_softmax(S, scale, g, t, Ph, Pm);
     } else {
-      // ---------------- O[chunk] = P V[chunk] ----------------
-      // V arrives pre-split in 8-channel groups [4 hi words | 4 mid words]; ldmatrix.trans turns the [key][channel]
-      // rows into the (k = key pair, n = channel) B fragments: matrices 0/1 = keys 0-7 / 8-15 hi, 2/3 = the mid parts.
+      // ---- re-lay the V chunk: (key 2i, key 2i+1 of a halo row) x channel -> (hi, mid) ----
+      for (int i = tid; i < MT_ROWS * (MT_COLS / 2) * MCH; i += 256) {
+        const int c = i & (MCH - 1), pr = i >> 5;               // pr = row * 12 + pair
+        const int px = (pr / (MT_COLS / 2)) * MT_COLS + (pr % (MT_COLS / 2)) * 2;
+        const float v0 = buf[px * BSTR + c], v1 = buf[(px + 1) * BSTR + c];
+        *reinterpret_cast<uint2*>(vpk + pr * VPSTR + 2 * c) = split_bf16x2(v0, v1);
+      }
+      __syncthreads();
       float O[MCH / 8][4];
-#pragma unroll
-      for (int nb = 0; nb < MCH / 8; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
-      const uint32_t vbase = (uint32_t)__cvta_generic_to_shared(buf) +
-                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * 4) * 4);
+      zero_acc(O);
 #pragma unroll
       for (int r = 0; r < 10; ++r) {
-        uint32_t bh0[MCH / 8], bh1[MCH / 8], bm0[MCH / 8], bm1[MCH / 8];
+        const uint32_t* vp = vpk + ((wy + r) * (MT_COLS / 2) + wx / 2 + t) * VPSTR + 2 * g;
+        uint2 b0[MCH / 8], b1[MCH / 8];
 #pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb)
-          asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-                       : "=r"(bh0[nb]), "=r"(bh1[nb]), "=r"(bm0[nb]), "=r"(bm1[nb])
-                       : "r"(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * 8) * 4)));
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Pm[r], bh0[nb], bh1[nb]);
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph[r], bm0[nb], bm1[nb]);
-#pragma unroll
-        for (int nb = 0; nb < MCH / 8; ++nb) mma_bf16(O[nb], Ph[r], bh0[nb], bh1[nb]);
-      }
-      const int cbase = (stage - nchunk) * MCH;
-      const int qx = x0 + wx + g;
-      if (qx < W) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int qy = y0 + wy + half;
-          if (qy < H) {
-            float* o = out + (img_off + (size_t)qy * W + qx) * ldo + cbase + 2 * t;
-#pragma unroll
-            for (int nb = 0; nb < MCH / 8; ++nb)
-              *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
-          }
+        for (int nb = 0; nb < MCH / 8; ++nb) {
+          b0[nb] = *reinterpret_cast<const uint2*>(vp + nb * 16);
+          b1[nb] = *reinterpret_cast<const uint2*>(vp + 4 * VPSTR + nb * 16);
         }
+        pv_row(O, Ph[r], Pm[r], b0, b1);
       }
+      store_patch(O, out, ldo, n, H, W, y0 + wy, x0 + wx + g, (stage - nchunk) * MCH, t);
     }
     __syncthreads();
   }
 }
 
 // ------------------------------------------------------------------------------------------------
-// PLANAR operands (split kind 3, C = 128: per pixel 64 hi words | 64 mid words; lcab_proj.cu writes them): the same
-// per-warp math as the kernel above -- 2 x 8 query patch and 10 x 16 key region per warp, k16 steps over 32-channel
-// chunks, the three split products in the order mid.hi, hi.mid, hi.hi, the same softmax and P V key grouping -- so the
-// results are bit-identical to it on the same hi / mid words.  What differs is how the operands arrive:
+// Interleaved PRE-SPLIT operands (di_lcab_window_pre_f32): q, k (kind 1) and v (kind 2) were written by the producing
+// dense layer's epilogue already as bf16 (hi, mid) words (gemm_tc.cu), 4 bytes per value at the value's own position.
+// No conversion pass, no packed-V buffer and one barrier less per stage: stages go straight from cp.async to fragments
+// (LDS.64 for Q/K; for V, which arrives in 8-channel groups [4 hi words | 4 mid words], ldmatrix.x4.trans).
+// ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(256, 1)
+lcab_window_pre_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk,
+                       const float* __restrict__ v, int ldv, float* __restrict__ out, int ldo, int H, int W, int C,
+                       float scale) {
+  extern __shared__ __align__(16) float smem[];   // [2][BSTAGE_WORDS]: K,Q chunk (pixel stride 40 words) or V chunk (36)
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int g = lane >> 2, t = lane & 3;
+  const int x0 = blockIdx.x * MQ_COLS, y0 = blockIdx.y * MQ_ROWS, n = blockIdx.z;
+  const size_t img_off = (size_t)n * H * W;
+  const int nchunk = C / MCH;
+  const int nstage = 2 * nchunk;
+  auto issue = [&](int stage) {
+    const bool is_k = stage < nchunk;
+    stage_chunk(smem + (stage & 1) * BSTAGE_WORDS, is_k ? k : v, is_k ? ldk : ldv, is_k ? BSTR : VSTR2,
+                is_k ? q : nullptr, ldq, (is_k ? stage : stage - nchunk) * MCH, img_off, x0, y0, H, W, tid);
+  };
+
+  const int wy = 2 * (warp >> 1), wx = 8 * (warp & 1);
+  float S[20][4];
+  zero_acc(S);
+  uint32_t Ph[10][4], Pm[10][4];                     // P = softmax(S) as packed bf16 hi / mid A fragments
+
+  issue(0);
+  for (int stage = 0; stage < nstage; ++stage) {
+    if (stage + 1 < nstage) {
+      issue(stage + 1);
+      cp_async_wait<1>();
+    } else {
+      cp_async_wait<0>();
+    }
+    __syncthreads();
+    float* buf = smem + (stage & 1) * BSTAGE_WORDS;
+    if (stage < nchunk) {
+      const uint32_t* kw = reinterpret_cast<const uint32_t*>(buf);
+      qk_chunk_interleaved(S, kw, kw + BKV_WORDS + (wy * MQ_COLS + wx) * BSTR, wy, wx, g, t);
+      if (stage == nchunk - 1) window_softmax(S, scale, g, t, Ph, Pm);
+    } else {
+      float O[MCH / 8][4];
+      zero_acc(O);
+      const uint32_t vbase = (uint32_t)__cvta_generic_to_shared(buf) +
+                             (uint32_t)(((wy * MT_COLS + wx + (lane & 7) + ((lane >> 3) & 1) * 8) * VSTR2 + (lane >> 4) * 4) * 4);
+#pragma unroll
+      for (int r = 0; r < 10; ++r) {
+        uint2 b0[MCH / 8], b1[MCH / 8];
+#pragma unroll
+        for (int nb = 0; nb < MCH / 8; ++nb) ldsm_v(vbase + (uint32_t)((r * MT_COLS * VSTR2 + nb * 8) * 4), b0[nb], b1[nb]);
+        pv_row(O, Ph[r], Pm[r], b0, b1);
+      }
+      store_patch(O, out, ldo, n, H, W, y0 + wy, x0 + wx + g, (stage - nchunk) * MCH, t);
+    }
+    __syncthreads();
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
+// PLANAR operands (split kind 3, C = 128: per pixel 64 hi words | 64 mid words; lcab_proj.cu writes them), the product
+// path.  window_core as in the kernels above; what differs is how the operands arrive:
 //   persistent grid: min(tiles, SMs) CTAs walk the 8 x 16 query tiles with a static stride in (image, band, column)
 //     order (no atomic tile counter: graphs on concurrent streams must not share scheduler state);
 //   TMA: per stage one elected thread loads the hi and the mid plane of the 32-channel chunk -- K (16 x 24 halo) and Q
@@ -862,8 +599,7 @@ lcab_window_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
     const int n = tile / per_image, rem = tile - n * per_image;
     const int y0 = (rem / cols) * MQ_ROWS, x0 = (rem % cols) * MQ_COLS;
     float S[20][4];
-#pragma unroll
-    for (int b = 0; b < 20; ++b) S[b][0] = S[b][1] = S[b][2] = S[b][3] = 0.f;
+    zero_acc(S);
     uint32_t Ph[10][4], Pm[10][4];
 
 #pragma unroll 1
@@ -881,22 +617,11 @@ lcab_window_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
         ah[1] = ld32(qb + MQ_COLS * 64 + f0);        am[1] = ld32(qb + TC_Q_PLANE + MQ_COLS * 64 + f0);
         ah[2] = ld32(qb + f1);                       am[2] = ld32(qb + TC_Q_PLANE + f1);
         ah[3] = ld32(qb + MQ_COLS * 64 + f1);        am[3] = ld32(qb + TC_Q_PLANE + MQ_COLS * 64 + f1);
-#pragma unroll
-        for (int r2 = 0; r2 < 5; ++r2) {
-          uint2 b0[4], b1[4];                        // (hi, mid) of the B fragment's two k halves
-#pragma unroll
-          for (int u = 0; u < 4; ++u) {
-            const uint32_t kp = kb + ((2 * r2 + (u >> 1)) * MT_COLS + (u & 1) * 8) * 64;
-            b0[u] = make_uint2(ld32(kp + f0), ld32(kp + TC_KV_PLANE + f0));
-            b1[u] = make_uint2(ld32(kp + f1), ld32(kp + TC_KV_PLANE + f1));
-          }
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], am, b0[u].x, b1[u].x);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].y, b1[u].y);
-#pragma unroll
-          for (int u = 0; u < 4; ++u) mma_bf16(S[r2 * 4 + u], ah, b0[u].x, b1[u].x);
-        }
+        qk_step(S, ah, am, [&](int b, uint2& b0, uint2& b1) {
+          const uint32_t kp = kb + ((b >> 1) * MT_COLS + (b & 1) * 8) * 64;
+          b0 = make_uint2(ld32(kp + f0), ld32(kp + TC_KV_PLANE + f0));
+          b1 = make_uint2(ld32(kp + f1), ld32(kp + TC_KV_PLANE + f1));
+        });
       }
       release();
       if (j == 3) window_softmax(S, scale, g, t, Ph, Pm);
@@ -907,39 +632,18 @@ lcab_window_tc_kernel(const __grid_constant__ CUtensorMap mapQ, const __grid_con
       // ---------------- O[chunk] = P V[chunk] ----------------
       if (tid == 0) produce();
       tc::mbar_wait(full(slot), phase);
-      float O[4][4];
-#pragma unroll
-      for (int nb = 0; nb < 4; ++nb) O[nb][0] = O[nb][1] = O[nb][2] = O[nb][3] = 0.f;
+      float O[MCH / 8][4];
+      zero_acc(O);
       const uint32_t vb = base + slot * TC_SLOT + (wy * MT_COLS + wx) * 64;
 #pragma unroll
       for (int r = 0; r < 10; ++r) {
-        uint32_t bh0[4], bh1[4], bm0[4], bm1[4];
+        uint2 b0[MCH / 8], b1[MCH / 8];
 #pragma unroll
-        for (int nb = 0; nb < 4; ++nb)
-          asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
-                       : "=r"(bh0[nb]), "=r"(bh1[nb]), "=r"(bm0[nb]), "=r"(bm1[nb])
-                       : "r"(vb + r * MT_COLS * 64 + (vl ^ (nb << 4))));
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Pm[r], bh0[nb], bh1[nb]);
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Ph[r], bm0[nb], bm1[nb]);
-#pragma unroll
-        for (int nb = 0; nb < 4; ++nb) mma_bf16(O[nb], Ph[r], bh0[nb], bh1[nb]);
+        for (int nb = 0; nb < MCH / 8; ++nb) ldsm_v(vb + r * MT_COLS * 64 + (vl ^ (nb << 4)), b0[nb], b1[nb]);
+        pv_row(O, Ph[r], Pm[r], b0, b1);
       }
       release();
-      const int qx = x0 + wx + g;
-      if (qx < W) {
-#pragma unroll
-        for (int half = 0; half < 2; ++half) {
-          const int qy = y0 + wy + half;
-          if (qy < H) {
-            float* o = out + ((size_t)(n * H + qy) * W + qx) * ldo + j * MCH + 2 * t;
-#pragma unroll
-            for (int nb = 0; nb < 4; ++nb)
-              *reinterpret_cast<float2*>(o + nb * 8) = make_float2(O[nb][half * 2], O[nb][half * 2 + 1]);
-          }
-        }
-      }
+      store_patch(O, out, ldo, n, H, W, y0 + wy, x0 + wx + g, j * MCH, t);
     }
   }
 }
@@ -963,7 +667,7 @@ bool window_map(CUtensorMap* m, const void* ptr, int ld, int N, int H, int W, in
 // Unfused NCHW window ops with the exact contract of the reference extension `localattention`
 // (locatt_ops/kernels.cuh: cc2k :4-42, ck2c_ori :44-80, ck2c_loc :82-119; fp32 data, fp64 accumulate
 // as in f_cc2k<float,double>).  They exist for drop-in compatibility (autograd of the unfused path);
-// the product forward uses lcab_window_kernel above.
+// the product forward uses the fused window kernels above.
 // ------------------------------------------------------------------------------------------------
 __global__ void locatt_cc2k_kernel(const float* __restrict__ x_ori, const float* __restrict__ x_loc,
                                    float* __restrict__ y, int C, int H, int W, int kH, int kW, long long total) {
@@ -1025,12 +729,13 @@ __global__ void locatt_ck2c_loc_kernel(const float* __restrict__ x_ori, const fl
 
 }  // namespace
 
-static int g_force_ffma_window = 0;   // 1: FFMA kernel, 2: 3xTF32 mma.sync kernel, 0: bf16-split mma.sync kernel
+static int g_force_ffma_window = 0;   // 1: di_lcab_window_f32 always runs the FFMA kernel
 
 extern "C" {
 
-// test hook: 0 = bf16-split tensor-core kernel (default), 1 = FFMA kernel, 2 = 3xTF32 tensor-core kernel
+// test hook: 0 = di_lcab_window_f32 picks its kernel (default), 1 = always the FFMA kernel
 int di_set_window_ffma(int on) {
+  DI_CHECK_ARG(on == 0 || on == 1, "di_set_window_ffma: expected 0 or 1 (got %d)", on);
   g_force_ffma_window = on;
   return DI_OK;
 }
@@ -1112,15 +817,6 @@ int di_lcab_window_f32(const float* q, int ldq, const float* k, int ldk, const f
       return DI_ERR_LAUNCH;
     }
     lcab_window_bf16_kernel<<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, scale);
-  } else if (ksize == 9 && C % MCH == 0 && g_force_ffma_window == 2) {
-    dim3 mgrid(di_cdiv(W, MQ_COLS), di_cdiv(H, MQ_ROWS), N);
-    size_t smem = 2ull * MSTAGE_FLOATS * sizeof(float);
-    static DiSmemOnce once_mma{};
-    if (!di_smem_once(once_mma, lcab_window_mma_kernel, (int)smem)) {
-      di_set_error("di_lcab_window_f32: cannot reserve shared memory");
-      return DI_ERR_LAUNCH;
-    }
-    lcab_window_mma_kernel<<<mgrid, 256, smem, stream>>>(q, ldq, k, ldk, v, ldv, out, ldo, H, W, C, scale);
   } else if (ksize == 9) {
     size_t smem = 2ull * (TQ + 8) * (TQ + 8) * PSTR * sizeof(float);
     static DiSmemOnce once9{};

@@ -16,12 +16,8 @@
 // items (alternating) and take turns on the tensor cores, so one warpgroup's epilogue runs under the other's MMA.  The
 // epilogue writes the output words into the item's own x stage (128-byte swizzle) and one thread stores the tile by
 // TMA.  Every layer issues the same k-steps with the same three split products in the same order as the bf16-split
-// GEMM (gemm_tc.cu), and the stored words are the same, so the results equal the five-launch chain bit for bit.
-//
-// Chain (di_lcab_proj_set_mode(0)): five launches of the bf16-split GEMM, each the same launch the unfused path makes.
-// The first-stage activations q1 / k1 are written into the q / k output buffers and the second stage runs IN PLACE
-// over them: with N = 128 there is one column tile, and a CTA has read all A rows of a tile (every K chunk) before its
-// epilogue writes that tile's rows, while no other CTA touches those rows.
+// GEMM (gemm_tc.cu), and the stored words are the same, so the results equal the five layers run as separate
+// di_linear_tcb_split_f32 launches bit for bit (tests/lcab_chain.py).
 #include "tc_common.cuh"
 #include "di_b200.h"
 
@@ -262,7 +258,6 @@ void role_split(int sms, int items, int* nq, int* nk, int* nv) {
 
 constexpr int MAX_DEV = 64;
 bool g_attr_set[MAX_DEV];
-int g_fused = 1;
 
 int proj_fused(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
                const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
@@ -302,39 +297,9 @@ int proj_fused(const float* x_t, int ld_t, const float* x_s, int ld_s, const voi
   return DI_OK;
 }
 
-int proj_chain(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
-               const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
-               int M, cudaStream_t stream) {
-  constexpr size_t WB = 128 * 128 * 2;               // bytes of one 128 x 128 bf16 weight block
-  auto w = [&](const void* p, int blk) { return static_cast<const void*>(static_cast<const char*>(p) + blk * WB); };
-  struct Layer {
-    const float* a; int lda; const void* wh; const void* wm; const float* b; float* out; int kind;
-  };
-  const Layer chain[5] = {
-      {x_t, ld_t, w(W1_hi, 0), w(W1_mid, 0), b1, q, 0},            // q1 = relu(W_q1 x_t + b_q1)  -> q (fp32)
-      {q, 128, w(W2_hi, 0), w(W2_mid, 0), b2, q, 3},               // q  = relu(W_q2 q1 + b_q2)   -> q (planar, in place)
-      {x_s, ld_s, w(W1_hi, 1), w(W1_mid, 1), b1 + 128, k, 0},      // k1 = relu(W_k1 x_s + b_k1)  -> k (fp32)
-      {k, 128, w(W2_hi, 1), w(W2_mid, 1), b2 + 128, k, 3},         // k  = relu(W_k2 k1 + b_k2)   -> k (planar, in place)
-      {x_s, ld_s, w(W1_hi, 2), w(W1_mid, 2), b1 + 256, v, 3},      // v  = relu(W_v x_s + b_v)    -> v (planar)
-  };
-  for (const Layer& l : chain) {
-    const int rc = di_linear_tcb_split_f32(l.a, l.lda, 128, nullptr, 0, 0, nullptr, 0, 0, l.wh, l.wm, l.b, nullptr, 0, 0,
-                                           l.out, 128, M, 128, DI_ACT_RELU, 0, l.kind, stream);
-    if (rc != DI_OK) return rc;
-  }
-  return DI_OK;
-}
-
 }  // namespace
 
 extern "C" {
-
-// 1 (default): the fused kernel; 0: the five-launch chain (A/B runs and tests)
-int di_lcab_proj_set_mode(int mode) {
-  DI_CHECK_ARG(mode == 0 || mode == 1, "di_lcab_proj_set_mode: mode must be 0 or 1");
-  g_fused = mode;
-  return DI_OK;
-}
 
 int di_lcab_proj_grid(int M, int* nq, int* nk, int* nv) {
   DI_CHECK_ARG(M > 0 && nq && nk && nv, "di_lcab_proj_grid: bad argument");
@@ -357,7 +322,7 @@ int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, con
   DI_CHECK_ARG((((uintptr_t)x_t | (uintptr_t)x_s | (uintptr_t)W1_hi | (uintptr_t)W1_mid | (uintptr_t)W2_hi | (uintptr_t)W2_mid |
                  (uintptr_t)q | (uintptr_t)k | (uintptr_t)v) & 15) == 0, "di_lcab_proj_f32: pointers must be 16-byte aligned");
   DI_CHECK_ARG(q != k && q != v && k != v, "di_lcab_proj_f32: q, k, v must be distinct buffers");
-  return (g_fused ? proj_fused : proj_chain)(x_t, ld_t, x_s, ld_s, W1_hi, W1_mid, b1, W2_hi, W2_mid, b2, q, k, v, M, stream);
+  return proj_fused(x_t, ld_t, x_s, ld_s, W1_hi, W1_mid, b1, W2_hi, W2_mid, b2, q, k, v, M, stream);
 }
 
 // LocalContextAttentionBlock.forward (models/utils/encoder_utils.py:119-135) for C = 128 as ONE call: the projections

@@ -111,32 +111,31 @@ def _pack_lcab(blk, device):
 
 
 def lcab_forward(pk, target, source, N, H, W):
-    """target/source: [N*H*W, C] pixel-major rows (same tensor object => self attention).
+    """target/source: [N*H*W, C] pixel-major row views (same tensor object => self attention).
     Where the tensor-core path applies, the projections that feed the window kernel write its operand format
-    directly (bf16 hi/mid words, ops.linear_split), so the window kernel has no conversion work."""
+    directly (bf16 hi/mid words), so the window kernel has no conversion work."""
     C = pk['C']
+    if ops.can_window_tc(N * H * W, C, pk['ks']):
+        # one C-ABI call: the fused projections (lcab_proj.cu), then the planar window kernel; the rows go in through
+        # their leading dimension, a view whose rows are not 16-byte aligned as a contiguous copy
+        aligned = lambda x: x.stride(1) == 1 and x.stride(0) >= C and x.stride(0) % 4 == 0 and x.data_ptr() % 16 == 0
+        t = target if aligned(target) else target.contiguous()
+        s = t if source is target else source if aligned(source) else source.contiguous()
+        return ops.lcab_forward_tc(t, s, pk['w_self'], pk['b_self'], pk['w_2'], pk['b_2'], N, H, W)
     pre = ops.can_presplit(N * H * W, C, pk['ks'])
-    tc = ops.can_window_tc(N * H * W, C, pk['ks'])       # planar window kernel: planar operands (split kind 3)
-    if tc and ops.LCAB_PROJ[0] and target.is_contiguous() and source.is_contiguous():
-        # one C-ABI call: the five projections (lcab_proj.cu), then the window kernel
-        return ops.lcab_forward_tc(target, source, pk['w_self'], pk['b_self'], pk['w_2'], pk['b_2'], N, H, W)
     if target is source:
         if pre:
-            t = ops.linear_split([source], pk['w_self'], pk['b_self'], ops.ACT_RELU, 2 * C, 3 if tc else 2)    # q1 | k1 | v(split)
+            t = ops.linear_split([source], pk['w_self'], pk['b_self'], ops.ACT_RELU, 2 * C, 2)    # q1 | k1 | v(split)
         else:
             t = ops.linear([source], pk['w_self'], pk['b_self'], ops.ACT_RELU)        # [M, 3C] = q1 | k1 | v
         q1, k1, v = t[:, :C], t[:, C:2 * C], t[:, 2 * C:]
     else:
         q1 = ops.linear([target], pk['w_q1'], pk['b_q1'], ops.ACT_RELU)
         if pre:
-            t = ops.linear_split([source], pk['w_kv1'], pk['b_kv1'], ops.ACT_RELU, C, 3 if tc else 2)          # k1 | v(split)
+            t = ops.linear_split([source], pk['w_kv1'], pk['b_kv1'], ops.ACT_RELU, C, 2)          # k1 | v(split)
         else:
             t = ops.linear([source], pk['w_kv1'], pk['b_kv1'], ops.ACT_RELU)          # [M, 2C] = k1 | v
         k1, v = t[:, :C], t[:, C:]
-    if tc:
-        q = ops.linear_split([q1], pk['w_q2'], pk['b_q2'], ops.ACT_RELU, 0, 3)
-        k = ops.linear_split([k1], pk['w_k2'], pk['b_k2'], ops.ACT_RELU, 0, 3)
-        return ops.lcab_window_tc(q, k, v, N, H, W, C)
     if pre:
         q = ops.linear_split([q1], pk['w_q2'], pk['b_q2'], ops.ACT_RELU, 0, 1)
         k = ops.linear_split([k1], pk['w_k2'], pk['b_k2'], ops.ACT_RELU, 0, 1)

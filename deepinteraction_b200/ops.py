@@ -179,12 +179,9 @@ def linear_split(srcs, W, bias, act, split_col0, split_kind):
     return out
 
 
-WINDOW_TC = [os.environ.get('DI_B200_WINDOW_TC', '1') != '0']   # planar-operand window kernel (C == 128) instead of the interleaved one
-
-
 def can_window_tc(M, C, ksize):
-    """True when the LCAB projections may emit planar operands for the planar window kernel (lcab.cu)."""
-    return bool(WINDOW_TC[0] and can_presplit(M, C, ksize) and C == 128)
+    """True when LocalContextAttentionBlock runs as lcab_forward_tc (fused projections + planar window kernel)."""
+    return bool(can_presplit(M, C, ksize) and C == 128)
 
 
 def lcab_window_tc(q, k, v, N, H, W, C, out=None):
@@ -197,37 +194,23 @@ def lcab_window_tc(q, k, v, N, H, W, C, out=None):
     return out
 
 
-LCAB_PROJ = [os.environ.get('DI_B200_LCAB_PROJ', '1') != '0']   # projection call (lcab_proj.cu) in front of the planar window kernel
-LCAB_FUSED = [True]   # the library's default mode
-
-
-def set_lcab_fused(on):
-    """Projections of lcab_proj / lcab_forward_tc as one fused kernel (True) or five GEMM launches (False); process-wide."""
-    _lib.check(_lib.lib().di_lcab_proj_set_mode(int(bool(on))), 'di_lcab_proj_set_mode')
-    LCAB_FUSED[0] = bool(on)
-
-
-if os.environ.get('DI_B200_LCAB_FUSED', '1') == '0':
-    set_lcab_fused(False)
-
-
 def lcab_proj(x_t, x_s, w1, b1, w2, b2):
-    """q, k, v (planar operands of lcab_window_tc) from the target / source rows in one call (one fused launch, or five
-    GEMM launches, see set_lcab_fused): w1 = Weight of [q1 | k1 | v] (384 x 128), w2 = Weight of [q2 | k2] (256 x 128),
-    BN folded."""
+    """q, k, v (planar operands of lcab_window_tc) from the target / source rows in one fused launch: w1 = Weight of
+    [q1 | k1 | v] (384 x 128), w2 = Weight of [q2 | k2] (256 x 128), BN folded."""
     M = x_t.shape[0]
     assert x_t.shape[1] == 128 and x_s.shape == x_t.shape and w1.shape == (384, 128) and w2.shape == (256, 128)
     out = torch.empty(3, M, 128, device=x_t.device, dtype=torch.float32)
     (pt, lt), (ps, ls) = _rows(x_t), _rows(x_s)
     _call('di_lcab_proj_f32', pt, lt, ps, ls, _ptr(w1.bh), _ptr(w1.bm), _ptr(b1), _ptr(w2.bh), _ptr(w2.bm), _ptr(b2),
           _ptr(out[0]), _ptr(out[1]), _ptr(out[2]), M, _stream(),
-          nbytes=4 * M * 128 * (4 if x_t is x_s else 5), flops=2 * 5 * M * 128 * 128, launches=1 if LCAB_FUSED[0] else 5)
+          nbytes=4 * M * 128 * (4 if x_t is x_s else 5), flops=2 * 5 * M * 128 * 128)
     return out[0], out[1], out[2]
 
 
 def lcab_forward_tc(x_t, x_s, w1, b1, w2, b2, N, H, W):
-    """LocalContextAttentionBlock for C = 128 in one C-ABI call (projection chain + planar window kernel).  The byte count
-    is the MODULE-boundary one of SURVEY.md 8(d): each distinct input map read once, the output written once."""
+    """LocalContextAttentionBlock for C = 128 in one C-ABI call (fused projections + planar window kernel).  x_t / x_s:
+    row views with 16-byte aligned rows (leading dimension % 4 == 0).  The byte count is the MODULE-boundary one of
+    SURVEY.md 8(d): each distinct input map read once, the output written once."""
     M = x_t.shape[0]
     assert M == N * H * W and x_t.shape[1] == 128 and x_s.shape == x_t.shape
     qkv = torch.empty(3, M, 128, device=x_t.device, dtype=torch.float32)
@@ -236,7 +219,7 @@ def lcab_forward_tc(x_t, x_s, w1, b1, w2, b2, N, H, W):
     _call('di_lcab_forward_f32', pt, lt, ps, ls, _ptr(w1.bh), _ptr(w1.bm), _ptr(b1), _ptr(w2.bh), _ptr(w2.bm), _ptr(b2),
           _ptr(qkv), _ptr(out), 128, N, H, W, _stream(),
           nbytes=4 * M * 128 * (2 if x_t is x_s else 3), flops=2 * 5 * M * 128 * 128 + 2 * 2 * 81 * M * 128,
-          launches=2 if LCAB_FUSED[0] else 6)
+          launches=2)
     return out
 
 

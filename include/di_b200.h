@@ -129,8 +129,6 @@ int di_lcab_window_tc_f32(const void* q, int ldq, const void* k, int ldk, const 
 int di_lcab_proj_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, const void* W1_hi, const void* W1_mid,
                      const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* q, float* k, float* v,
                      int M, cudaStream_t stream);
-/* 1 = the fused kernel (default), 0 = five separate bf16-split GEMM launches (process-wide; A/B runs and tests) */
-int di_lcab_proj_set_mode(int mode);
 /* CTAs per role (Q, K, V) the fused kernel launches for M rows under the current SM budget (di_tc_set_sm_limit) */
 int di_lcab_proj_grid(int M, int* nq, int* nk, int* nv);
 
@@ -140,9 +138,9 @@ int di_lcab_forward_f32(const float* x_t, int ld_t, const float* x_s, int ld_s, 
                         const float* b1, const void* W2_hi, const void* W2_mid, const float* b2, float* qkv, float* out, int ldo,
                         int N, int H, int W, cudaStream_t stream);
 
-/* test/diagnostic hook: 1 = always use the FFMA window kernel, 0 = tensor-core (mma.sync 3xTF32) kernel when
- * ksize == 9 and C % 32 == 0 (default) */
-int di_set_window_ffma(int on); /* test hook: 0 = bf16-split mma.sync kernel (default), 1 = FFMA, 2 = 3xTF32 mma.sync */
+/* test/diagnostic hook for di_lcab_window_f32: 0 = the bf16-split mma.sync kernel when ksize == 9 and C % 32 == 0,
+ * else FFMA (default); 1 = always the FFMA kernel.  Other values are rejected. */
+int di_set_window_ffma(int on);
 
 /* The reference extension's own five entry points, unfused and NCHW, for drop-in compatibility
  * (locatt_ops/localAttention.cpp:61-73): similar_forward = cc2k(x_ori, x_loc); weighting_forward =

@@ -5,7 +5,7 @@ on the seeded inputs of tests/locatt_cases.py):
   (i)   the five drop-in entry points of projects/.../locatt_ops (forward + the three backward mappings, served by
         di_locatt_{cc2k,ck2c_ori,ck2c_loc}_f32) == the reference functions (localAttention.cpp:61-73), incl. non-square
         maps and kH != kW;
-  (ii)  the fused window kernels (planar bf16 split, mma.sync 3xTF32 / bf16 split, FFMA) == reference
+  (ii)  the fused window kernels (planar, interleaved pre-split and fp32-operand bf16 split, FFMA) == reference
         similar_forward -> softmax(./sqrt(C)) -> weighting_forward (encoder_utils.py:132-134);
   (iii) the CPU oracle's window ops == the reference kernels (this pins the one op whose committed golden had to use a
         stand-in, SURVEY.md Appendix B).
@@ -78,7 +78,7 @@ def test_drop_in_backward_is_the_gradient_of_the_forward():
         assert rel_err(a.cpu().double(), b) < 2e-5, name
 
 
-@pytest.mark.parametrize('kernel', ['planar', 'mma-bf16split', 'mma-3xtf32', 'ffma'])
+@pytest.mark.parametrize('kernel', ['planar', 'mma-pre', 'mma-bf16split', 'ffma'])
 @pytest.mark.parametrize('N,H,W', lc.FUSED)
 def test_fused_window_equals_reference_similar_softmax_weighting(ref, kernel, N, H, W):
     from deepinteraction_b200 import ops, fold, _lib
@@ -88,8 +88,11 @@ def test_fused_window_equals_reference_similar_softmax_weighting(ref, kernel, N,
     if kernel == 'planar':
         out = ops.lcab_window_tc(fold.split_rows(rows(q), 3), fold.split_rows(rows(kk), 3), fold.split_rows(rows(v), 3),
                                  N, H, W, C)
+    elif kernel == 'mma-pre':
+        out = ops.lcab_window_pre(fold.split_rows(rows(q), 1), fold.split_rows(rows(kk), 1), fold.split_rows(rows(v), 2),
+                                  N, H, W, C)
     else:
-        _lib.lib().di_set_window_ffma({'mma-bf16split': 0, 'ffma': 1, 'mma-3xtf32': 2}[kernel])
+        _lib.lib().di_set_window_ffma({'mma-bf16split': 0, 'ffma': 1}[kernel])
         try:
             out = ops.lcab_window(rows(q), rows(kk), rows(v), N, H, W, C, k)
         finally:

@@ -1,9 +1,10 @@
-"""GPU: the planar 9x9 window kernel (di_lcab_window_tc_f32, C = 128) against the interleaved pre-split kernel
-(di_lcab_window_pre_f32, q / k kind 1, v kind 2), bit for bit.
+"""GPU: the planar 9x9 window kernel (di_lcab_window_tc_f32, C = 128) and the fp32-operand kernel
+(di_lcab_window_f32, any C % 32 == 0) against the interleaved pre-split kernel (di_lcab_window_pre_f32, q / k kind 1,
+v kind 2), bit for bit.
 
-Both kernels feed the same bf16 hi / mid words into the same fragment algebra (2 x 8 query patch per warp, the same
+All three kernels feed the same bf16 hi / mid words into the same fragment algebra (2 x 8 query patch per warp, the same
 k16 steps, split products, softmax and P V key grouping), so only the operand layout and the way the operands reach
-shared memory differ.  The cases cover one tile, tiles cut by the image border, several images, non-contiguous row
+shared memory differ; the fp32-operand kernel splits in shared memory exactly as the dense layers' epilogue does.  The cases cover one tile, tiles cut by the image border, several images, non-contiguous row
 strides, persistent grids of 1, 3 and 7 CTAs (also with fewer tiles than CTAs), concurrent streams and CUDA-graph
 replays on two streams."""
 import os
@@ -34,10 +35,10 @@ def strided(x, pad):
     return view
 
 
-def inputs(N, H, W, seed):
+def inputs(N, H, W, seed, c=C):
     g = torch.Generator().manual_seed(seed)
     M = N * H * W
-    q, k, v = (torch.randn(M, C, generator=g).to(dev()) for _ in range(3))
+    q, k, v = (torch.randn(M, c, generator=g).to(dev()) for _ in range(3))
     return q * 1.7, k, v                               # logits spread over a few units after the 1/sqrt(C) scale
 
 
@@ -46,7 +47,7 @@ def planar(q, k, v, pad=0):
 
 
 def interleaved(q, k, v, N, H, W):
-    return ops.lcab_window_pre(fold.split_rows(q, 1), fold.split_rows(k, 1), fold.split_rows(v, 2), N, H, W, C)
+    return ops.lcab_window_pre(fold.split_rows(q, 1), fold.split_rows(k, 1), fold.split_rows(v, 2), N, H, W, q.shape[1])
 
 
 def window_tc(ops_in, N, H, W, out=None):
@@ -64,6 +65,15 @@ def test_planar_equals_interleaved(N, H, W, pad):
     if pad:                                            # the words around the written rows stay untouched
         base = got.as_strided((got.shape[0], C + 16), (C + 16, 1), got.storage_offset() - 8)
         assert torch.isnan(base[:, :8]).all() and torch.isnan(base[:, C + 8:]).all()
+
+
+@pytest.mark.parametrize('c', [32, 64, 128, 256])
+@pytest.mark.parametrize('N,H,W', SHAPES)
+def test_fp32_operands_equal_interleaved(N, H, W, c):
+    """The fp32-operand kernel (default for a 9x9 window and C % 32 == 0) == the interleaved kernel on split_rows of the
+    same rows."""
+    q, k, v = inputs(N, H, W, 300 + H + W + c, c)
+    assert torch.equal(i32(ops.lcab_window(q, k, v, N, H, W, c)), i32(interleaved(q, k, v, N, H, W)))
 
 
 @pytest.mark.parametrize('sms', [1, 3, 7, 0], ids=['sm1', 'sm3', 'sm7', 'nolimit'])

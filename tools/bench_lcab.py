@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Per-stage timing of LocalContextAttentionBlock (C = 128) at the base shapes: the projection stage (ops.lcab_proj)
-in both arms -- the fused kernel and the five-launch chain -- and the planar window kernel (ops.lcab_window_tc), each
-timed as separate calls with CUDA events, L2 flushed before every call.  Prints one JSON line per shape.
+"""Per-stage timing of LocalContextAttentionBlock (C = 128) at the base shapes: the projection stage in both arms --
+the fused kernel (ops.lcab_proj) and the five-launch chain of tests/lcab_chain.py -- and the planar window kernel
+(ops.lcab_window_tc), each timed as separate calls with CUDA events, L2 flushed before every call.  Prints one JSON line
+per shape.
 
 Projection rates are quoted against the fused floor: each distinct input map read once and q, k, v written once,
 4 F bytes for self attention and 5 F for cross attention (F = M * 128 * 4 bytes).  The peak is the H100 SXM data-sheet
@@ -28,6 +29,7 @@ import torch
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
+sys.path.append(os.path.join(ROOT, 'tests'))
 
 
 def timed(fn, flush, iters):
@@ -67,6 +69,7 @@ def main():
     ap.add_argument('--only', default='')
     args = ap.parse_args()
     from deepinteraction_b200 import _lib, mmri, ops, synth
+    from lcab_chain import chain
     dev = torch.device('cuda:0')
     torch.set_grad_enabled(False)
     peak, peak_src = 3350.0, 'H100 SXM data sheet (3.35 TB/s)'
@@ -97,17 +100,13 @@ def main():
         _lib.check(_lib.lib().di_lcab_proj_grid(M, *[ctypes.byref(r) for r in roles]), 'di_lcab_proj_grid')
         res['proj_fused_ctas_qkv'] = [r.value for r in roles]
         outs = {}
-        for arm, fused in (('fused', True), ('chain', False)):
-            ops.set_lcab_fused(fused)
-            us = timed(lambda: ops.lcab_proj(x, y, *w), flush, args.iters)
-            q, k, v = ops.lcab_proj(x, y, *w)
-            outs[arm] = (q, k, v)
+        for arm, fn in (('fused', lambda: ops.lcab_proj(x, y, *w)), ('chain', lambda: chain(x, y, *w))):
+            us = timed(fn, flush, args.iters)
+            outs[arm] = [t.view(torch.int32) for t in fn()]
             gbs = floor / (us * 1e-6) / 1e9
             res['proj_' + arm] = dict(us=round(us, 1), gbs_vs_floor=round(gbs, 1), frac_of_peak=round(gbs / peak, 3))
-        ops.set_lcab_fused(True)
-        res['fused_equals_chain'] = all(torch.equal(a.view(torch.int32), b.view(torch.int32))
-                                        for a, b in zip(outs['fused'], outs['chain']))
-        q, k, v = outs['fused']
+        res['fused_equals_chain'] = all(torch.equal(a, b) for a, b in zip(outs['fused'], outs['chain']))
+        q, k, v = (t.view(torch.float32) for t in outs['fused'])
         out = torch.empty(M, C, device=dev)
         res['window_us'] = round(timed(lambda: ops.lcab_window_tc(q, k, v, N, H, W, C, out=out), flush, args.iters), 1)
         win = window_counts(N, H, W, peak)

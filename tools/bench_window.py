@@ -1,4 +1,4 @@
-"""Times the window-attention kernels (0 = bf16-split mma.sync, 2 = 3xTF32 mma.sync, 1 = FFMA) at the bench shapes."""
+"""Times the kernels of di_lcab_window_f32 (0 = bf16-split mma.sync, 1 = FFMA) at the bench shapes."""
 import os, sys
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np
@@ -10,7 +10,7 @@ L = _lib.lib()
 junk = torch.empty(64 << 20, device=dev)
 for (N, H, W, C) in ((6, 112, 200, 128), (1, 180, 180, 128)):
     q, k, v = (torch.randn(N * H * W, C, device=dev) for _ in range(3))
-    for mode in (0, 2, 1):
+    for mode in (0, 1):
         L.di_set_window_ffma(mode)
         for _ in range(2):
             out = ops.lcab_window(q, k, v, N, H, W, C, 9)
