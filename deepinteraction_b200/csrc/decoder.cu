@@ -142,9 +142,30 @@ topk_kernel(const float* __restrict__ scores_all, const int* __restrict__ src_id
     }
   }
   __syncthreads();
-  // ties at the threshold: take the `need` smallest indices (a single thread; ties are measure-zero)
-  if (t == 0) {
-    unsigned ne = min(s_cnt_eq, (unsigned)TOPK_MAX);
+  if (s_cnt_eq > TOPK_MAX) {
+    // more ties than eq_idx holds (e.g. a row of zeros): block-wide pass over the slice in ascending index order, chunks of
+    // blockDim indices, each tie ranked by a ballot and a prefix count over the warps, until `need` of them are taken
+    __shared__ unsigned warp_cnt[32];
+    const int lane = t & 31, w = t >> 5, nw = blockDim.x >> 5;
+    for (unsigned taken = 0, base = 0; taken < need && base < (unsigned)n; base += blockDim.x) {
+      const unsigned i = base + t;
+      const bool hit = i < (unsigned)n && __float_as_uint(s[i]) == prefix;
+      const unsigned bal = __ballot_sync(0xffffffffu, hit);
+      if (lane == 0) warp_cnt[w] = __popc(bal);
+      __syncthreads();
+      unsigned rank = taken + __popc(bal & ((1u << lane) - 1u)), total = 0;
+      for (int j = 0; j < nw; ++j) {
+        if (j < w) rank += warp_cnt[j];
+        total += warp_cnt[j];
+      }
+      if (hit && rank < need)
+        cand[s_cnt_gt + rank] = ((unsigned long long)prefix << 32) | (unsigned long long)(0xffffffffu - i);
+      __syncthreads();
+      taken += total;
+    }
+  } else if (t == 0) {
+    // ties at the threshold: take the `need` smallest indices (a single thread; ties are measure-zero)
+    unsigned ne = s_cnt_eq;
     for (unsigned a = 0; a < need; ++a) {
       unsigned best = a;
       for (unsigned b2 = a + 1; b2 < ne; ++b2)
@@ -1330,7 +1351,7 @@ int di_heatmap_nms_f32(const float* a, const float* b, int ld, float* out, float
   return DI_OK;
 }
 
-// scores [B,n] >= 0 -> idx [B,k] (descending score, ties by ascending index); k <= 1024.
+// scores [B,n] >= 0 -> idx [B,k] (descending score, ties by ascending index, however many tie); k <= 1024.
 // work: B * slices * k * 2 ints/floats of scratch (pass nullptr/0 slices for the single-level path).
 int di_topk_f32(const float* scores, int* idx, int B, int n, int k, void* work, int slices, cudaStream_t stream) {
   DI_CHECK_ARG(scores && idx && B > 0 && n >= k && k > 0 && k <= TOPK_MAX, "di_topk_f32: bad argument (k=%d n=%d)", k, n);
@@ -1341,12 +1362,14 @@ int di_topk_f32(const float* scores, int* idx, int B, int n, int k, void* work, 
   }
   float* cval = reinterpret_cast<float*>(work);
   int* cidx = reinterpret_cast<int*>(cval + (size_t)B * slices * k);
-  int n_slice = di_cdiv(n, slices);
+  // no slice but the last is shorter than k: the index -1 pads of a short slice then trail every real candidate, and
+  // level 2 (ties by ascending candidate position) reaches them only after all real indices
+  int n_slice = max(di_cdiv(n, slices), k);
   slices = di_cdiv(n, n_slice);
   topk_kernel<<<dim3(slices, B), 1024, 0, stream>>>(scores, nullptr, n, n_slice, k, cval, cidx);
   DI_CHECK_LAUNCH("di_topk_f32(level 1)");
-  // level 2: candidates of empty tail slots carry value 0 / index -1 and can only win when fewer than k
-  // positive scores exist in the whole row
+  // level 2: candidates of empty tail slots carry value 0 / index -1; they sit after every real candidate, of which there
+  // are at least k, so they are never selected
   topk_kernel<<<dim3(1, B), 1024, 0, stream>>>(cval, cidx, slices * k, slices * k, k, nullptr, idx);
   DI_CHECK_LAUNCH("di_topk_f32(level 2)");
   return DI_OK;

@@ -241,7 +241,9 @@ int di_polar_gather_f32(const float* rays, const float* lidar, const float* proj
 /* models/dense_heads/deepinteraction_decoder.py:225-239 */
 int di_heatmap_nms_f32(const float* a, const float* b, int ld, float* out, float* dense_b, int B, int K, int H, int W,
                        int ks, int no_nms_class_mask, cudaStream_t stream);
-/* :242 (argsort descending, first k) */
+/* :242 (argsort descending, first k).  scores [B,n] >= 0 -> idx [B,k], 0 < k <= min(n, 1024): descending score, ties
+ * by ascending index however many tie at the cut, deterministic; every index is in [0, n).  work: float [2*B*slices*k]
+ * (NULL / slices <= 1: one level; slices are at least k long, so their number may come out smaller). */
 int di_topk_f32(const float* scores, int* idx, int B, int n, int k, void* work, int slices, cudaStream_t stream);
 /* :243-253, :299 */
 int di_query_init_f32(const float* feat, const int* top, const float* heat, const float* wce_t, const float* bce,

@@ -1,0 +1,35 @@
+"""Helpers of the kernel-level GPU tests: direct calls of the C entry points, the per-row error metric and bit equality.
+
+row_err takes the max over output rows of max|a-b| / scale_row, where scale_row is the magnitude of the terms summed into
+that row (>= max|b_row|).  A global max hides a wrong row whose values are small; and fp32 rounding is relative to the
+summed terms, not to their sum, which may cancel.  A row whose terms are all zero must be exactly zero."""
+import torch
+
+
+def _ops():
+    from deepinteraction_b200 import ops
+    return ops
+
+
+def _capi(name, *args):
+    """Call a C entry point directly (the wrappers allocate their outputs; these tests pre-fill them)."""
+    ops = _ops()
+    ops._call(name, *args, ops._stream())
+    torch.cuda.synchronize()
+
+
+def row_err(got, want, scale, width=None):
+    """max over rows of max|got - want| / max(scale_row, max|want_row|); rows are the last dimension, or groups of
+    `width` values of it."""
+    g, w, s = (t.detach().double().cpu() for t in (got, want, scale))
+    s = torch.broadcast_to(s, g.shape)
+    n = width or g.shape[-1]
+    g, w, s = g.reshape(-1, n), w.reshape(-1, n), s.reshape(-1, n)
+    den = torch.maximum(w.abs().amax(1), s.abs().amax(1))
+    err = (g - w).abs().amax(1)
+    return float(torch.where(den > 0, err / den.clamp_min(1e-300), err * 1e30).max())
+
+
+def same_bits(a, b):
+    a, b = a.detach().cpu().contiguous(), b.detach().cpu().contiguous()
+    return a.shape == b.shape and torch.equal(a.view(torch.int32), b.view(torch.int32))

@@ -22,6 +22,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_err
+from kernel_check import _capi, row_err, same_bits
 
 pytestmark = pytest.mark.gpu
 
@@ -41,30 +42,6 @@ def _ops():
 
 def _p(t):
     return _ops()._ptr(t)
-
-
-def _capi(name, *args):
-    """Call a C entry point directly (the wrappers allocate their outputs; these tests pre-fill them)."""
-    ops = _ops()
-    ops._call(name, *args, ops._stream())
-    torch.cuda.synchronize()
-
-
-def row_err(got, want, scale, width=None):
-    """max over rows of max|got - want| / max(scale_row, max|want_row|); rows are the last dimension, or groups of
-    `width` values of it."""
-    g, w, s = (t.detach().double().cpu() for t in (got, want, scale))
-    s = torch.broadcast_to(s, g.shape)
-    n = width or g.shape[-1]
-    g, w, s = g.reshape(-1, n), w.reshape(-1, n), s.reshape(-1, n)
-    den = torch.maximum(w.abs().amax(1), s.abs().amax(1))
-    err = (g - w).abs().amax(1)
-    return float(torch.where(den > 0, err / den.clamp_min(1e-300), err * 1e30).max())
-
-
-def same_bits(a, b):
-    a, b = a.detach().cpu().contiguous(), b.detach().cpu().contiguous()
-    return a.shape == b.shape and torch.equal(a.view(torch.int32), b.view(torch.int32))
 
 
 # ---------------------------------------------------------------------------------------------------------------------
