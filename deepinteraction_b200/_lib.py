@@ -111,6 +111,9 @@ SIGNATURES = {
     'di_rcnn_rois_f32': [_p, _i, _p, _p, _p, _p, _p, _i, _i, _i, _i, _fp, _p],
     'di_roi_align_f32': [_p, _p, _p, _i, _i, _i, _i, _f, _p],
     'di_dynconv_f32': [_p, _p, _p, _p, _p, _p, _p, _i, _f, _p],
+    'di_roi_align_bwd_f32': [_p, _p, _p, _i, _i, _i, _i, _i, _f, _p],
+    'di_dynconv_bwd_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _f, _p],
+    'di_gelu_bwd_f32': [_p, _p, _p, _ll, _p],
     'di_nchw_to_nhwc_f32': [_p, _p, _i, _i, _i, _p],
     'di_nhwc_to_nchw_f32': [_p, _p, _i, _i, _i, _p],
     'di_bbox_decode_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _f, _f, _f, _f, _fp, _f, _i, _p, _p, _p, _p, _p],

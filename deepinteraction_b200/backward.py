@@ -49,6 +49,8 @@ def _wgrad(dy, x):
     dyt = ops.nhwc_to_nchw(dy.view(1, M, 1, dy.shape[1])).view(dy.shape[1], M)
     xt = ops.nhwc_to_nchw(x.view(1, M, 1, x.shape[1])).view(x.shape[1], M)
     splits = max(1, min(256, M // 512))
+    if splits == 1:
+        return ops.linear([dyt], xt)
     part = ops.linear([dyt], xt, splits=splits)
     return ops.rows_finish(part) if part.shape[0] > 1 else part[0]
 
@@ -384,3 +386,122 @@ class DecoderLayerFunction(torch.autograd.Function):
         query, query_pos, bev = ctx.saved_tensors
         r = decoder_layer_backward(ctx.dec, query, query_pos, bev, grad_out)
         return None, r['d_query'], None, r['d_bev']
+
+
+# ---- decoder: PointRCNNBlock (the BEV refinement block of the MMPI layers) -----------------------------------------------
+def _rcnn_bw_pack(dec, bp, li):
+    """Transposed weights of the block's dX products, built once per pack.  The DynamicConv generator's transpose
+    [C, 2*128*128] stays a plain tensor: its dX product (K = 32768 over B*P rows) runs as a split-K FFMA product."""
+    if '_bw' in bp:
+        return bp['_bw']
+    blk = dec.decode_head[li]
+    g = lambda n: getattr(blk, n + blk.sfx)
+    dev = bp['norm1'][0].device
+    C = dec.hidden_channel
+    T = lambda w: fold.Weight(fold._d(w).t().contiguous(), dev)
+    s = float(C // dec.num_heads) ** -0.5
+    mha, dyn = g('dyconv_pre_self_attn'), g('dyconv')
+    w_in = fold._d(mha.in_proj_weight).clone()
+    w_in[:C] *= s                                   # the q rows _pack_mha folds the head_dim^-0.5 into
+    qscale = torch.cat([torch.full((C,), s, dtype=torch.float64), torch.ones(2 * C, dtype=torch.float64)])
+    bp['_bw'] = dict(ffn2=T(g('linear2').weight), ffn1=T(g('linear1').weight), dout=T(dyn.out_layer.weight),
+                     dyn=fold.dev(fold._d(dyn.dynamic_layer.weight).t(), dev), attn_out=T(mha.out_proj.weight),
+                     attn_in=fold.Weight(w_in.t().contiguous(), dev), qscale=fold.dev(qscale, dev))
+    return bp['_bw']
+
+
+# the dX product of the DynamicConv generator: d q1 [B*P, C] = d params [B*P, 32768] W_dyn.  The tensor-core GEMM has no
+# split-K, and at M ~ 200 - 400 rows and N = 128 it would run on 2 - 4 CTAs over the whole K; 64 splits of 512 give
+# 128 - 256 CTAs of the FFMA kernel, reduced in a fixed order by di_rows_finish_f32 together with the residual gradient.
+_DYN_SPLITS = 64
+
+
+def _point_rcnn_block(dec, li, query, bev):
+    """-> (block pack, B, P); NotImplementedError before any launch for what point_rcnn_backward does not cover."""
+    bp = dec.pack()['blocks'][li]
+    if bp['image'] or bp['v2']:
+        raise NotImplementedError('point_rcnn_backward covers the V1 PointRCNNBlock only (decode_head[%d] is %s)'
+                                  % (li, type(dec.decode_head[li]).__name__))
+    C, M, B = dec.hidden_channel, query.shape[0], bev.shape[0]
+    P = M // B
+    if C != 128 or bev.shape[3] != C or query.shape[1] != C or P > 512 or P * B != M:
+        raise NotImplementedError('point_rcnn_backward: C = 128 and P <= 512 queries per sample '
+                                  f'(got C={query.shape[1]}, rows={M}, B={B})')
+    return bp, B, P
+
+
+def _bev_roi_params(dec):
+    return dec._roi_params((0, 0))          # the image size enters the image-mode RoIs only
+
+
+def point_rcnn_backward(dec, li, query, pred, bev, grad_out):
+    """Backward of the base decoder's PointRCNNBlock (reference models/utils/decoder_utils.py:765-841; dec.decode_head[li],
+    li = 1 or 3 in the base configuration), LayerNorms as they are, dropout off.
+    dec: DeepInteractionDecoder on the GPU; query [B*P, C]: the rows the block reads; pred [B*P, NP]: the prediction rows its
+    RoIs come from (di_rcnn_rois_f32, BEV mode); bev [B, Y, X, C]: new_pts (pixel-major); grad_out [B*P, C].
+    -> dict(d_query [B*P, C], d_bev [B, Y, X, C] (through RoIAlign), grads = {name: tensor} for the 24 parameters of
+    dec.decode_head[li], keyed and shaped as in its state_dict).  The RoIs are constants (the reference computes them
+    from detached predictions), so pred gets no gradient.  The block is re-run eagerly with its intermediates kept;
+    everything stays on the device, without host synchronisation after the first call of a pack."""
+    bp, B, P = _point_rcnn_block(dec, li, query, bev)
+    with _precise():
+        return _point_rcnn_backward(dec, li, bp, query.contiguous(), pred.contiguous(), bev.contiguous(),
+                                    grad_out.contiguous(), B, P)
+
+
+def _point_rcnn_backward(dec, li, bp, query, pred, bev, grad_out, B, P):
+    C, H = dec.hidden_channel, dec.num_heads
+    _, Y, X, _ = bev.shape
+    sv = {}
+    dec._rcnn_block(bp, query, pred, bev, None, B, P, _bev_roi_params(dec), None, None, saved=sv)
+    bw = _rcnn_bw_pack(dec, bp, li)
+    R = {}
+    # norm3, FFN (GELU)
+    dz3, R['norm3_pts.weight'], R['norm3_pts.bias'] = ops.ln_bwd(grad_out, sv['z3'], bp['norm3'][0])
+    R['linear2_pts.weight'], R['linear2_pts.bias'] = _wgrad(dz3, sv['f']), ops.col_sum(dz3)
+    dh = ops.gelu_bwd(ops.linear([dz3], bw['ffn2']), sv['h'])
+    R['linear1_pts.weight'], R['linear1_pts.bias'] = _wgrad(dh, sv['q2']), ops.col_sum(dh)
+    dq2 = ops.linear([dh], bw['ffn1'], res=dz3)
+    # norm2, DynamicConv: norm3 + ReLU, out_layer, the dynamic convolution, the parameter generator, RoIAlign
+    dz2, R['norm2_pts.weight'], R['norm2_pts.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
+    D = 'dyconv_pts.'
+    dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
+    R[D + 'out_layer.weight'], R[D + 'out_layer.bias'] = _wgrad(dzd3, sv['flat']), ops.col_sum(dzd3)
+    d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
+    dn = ops.col_sum(d_norm).view(4, C)
+    R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
+    R[D + 'dynamic_layer.weight'], R[D + 'dynamic_layer.bias'] = _wgrad(d_params, sv['q1']), ops.col_sum(d_params)
+    dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
+    d_bev = ops.roi_align_bwd(d_roi, sv['rois'], B, Y, X, 1.0)
+    # norm1, self attention over the queries of a sample (BEV mode: one group, no masks)
+    dz1, R['norm1_pts.weight'], R['norm1_pts.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
+    A = 'dyconv_pre_self_attn_pts.'
+    R[A + 'out_proj.weight'], R[A + 'out_proj.bias'] = _wgrad(dz1, sv['a']), ops.col_sum(dz1)
+    qkv = sv['qkv']
+    dqkv = ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ops.linear([dz1], bw['attn_out']), B, P, H)
+    d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
+    # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
+    R[A + 'in_proj_weight'] = _wgrad(dqkv, query) * bw['qscale'][:, None]
+    R[A + 'in_proj_bias'] = ops.col_sum(dqkv) * bw['qscale']
+    return dict(d_query=d_query, d_bev=d_bev, grads=R)
+
+
+class PointRCNNFunction(torch.autograd.Function):
+    """autograd wrapper: out [B*P, C] = dec.decode_head[li] (a V1 PointRCNNBlock) with the forward schedule's kernels, bit
+    for bit; backward -> (d_query, d_bev) through point_rcnn_backward, no gradient for pred (the RoIs are constants).
+    Parameter gradients are returned by point_rcnn_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, li, query, pred, bev):
+        bp, B, P = _point_rcnn_block(dec, li, query, bev)
+        ctx.dec, ctx.li = dec, li
+        ctx.save_for_backward(query, pred, bev)
+        with _precise():
+            return dec._rcnn_block(bp, query.contiguous(), pred.contiguous(), bev.contiguous(), None, B, P,
+                                   _bev_roi_params(dec), None, None)[0]
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        query, pred, bev = ctx.saved_tensors
+        r = point_rcnn_backward(ctx.dec, ctx.li, query, pred, bev, grad_out)
+        return None, None, r['d_query'], None, r['d_bev']

@@ -1066,12 +1066,199 @@ roi_align_kernel(const float* __restrict__ maps, const float* __restrict__ rois,
 }
 
 // ------------------------------------------------------------------------------------------------
+// RoIAlign backward: d_maps [n_maps, H, W, C] from d_out [n, 49, C], as a gather (no atomics, deterministic).
+// The forward's bilinear weight is separable: pixel (py, px) receives from bin (ph, pw) the weight
+// Ay[ph](py) Ax[pw](px) / 4, where Ay[ph](py) sums over the bin's two y-samples that sample's row weight on py (0 for a
+// skipped sample) and Ax is the same along x.  A sample is skipped when y or x is out of [-1, L] or NaN, so the skip
+// factor of a sample is the product of a y and an x factor.  A CTA owns a 4 x 8 pixel tile of one map; it culls the RoI
+// list against the tile, 256 RoIs at a time, into an ascending list in shared memory; each warp owns 4 pixels of one tile
+// row (lanes over channels, the sums in registers) and adds the surviving RoIs in ascending RoI index, bins in ascending
+// order.  Pixels no sample reaches get exactly 0.
+// ------------------------------------------------------------------------------------------------
+constexpr int RB_TY = 4, RB_TX = 8, RB_PPW = 4, RB_T = 256;
+
+// One axis sample of roi_align_kernel (bin p, sub-sample i of 2; start a0, bin size bsz, L pixels): false when skipped,
+// else the two taps lo, hi (equal at the last pixel) and their weights.  The expressions are the forward's.
+__device__ __forceinline__ bool roi_axis_sample(float a0, float bsz, int p, int i, int L, int& lo, int& hi, float& wlo,
+                                                float& whi) {
+  float y = a0 + (float)p * bsz + ((float)i + 0.5f) * bsz / (float)2;
+  if (y < -1.f || y > (float)L) return false;
+  if (!(y == y)) return false;
+  y = fmaxf(y, 0.f);
+  lo = (int)y;
+  if (lo >= L - 1) { hi = lo = L - 1; y = (float)lo; } else hi = lo + 1;
+  const float l = y - (float)lo;
+  wlo = 1.f - l;
+  whi = l;
+  return true;
+}
+
+// weights a[p] of pixel q on the 7 bins of one axis
+__device__ __forceinline__ bool roi_axis_weights(float a0, float bsz, int L, int q, float (&a)[7]) {
+  bool any = false;
+#pragma unroll
+  for (int p = 0; p < 7; ++p) {
+    float s = 0.f;
+#pragma unroll
+    for (int i = 0; i < 2; ++i) {
+      int lo, hi;
+      float wl, wh;
+      if (roi_axis_sample(a0, bsz, p, i, L, lo, hi, wl, wh)) {
+        if (lo == q) s += wl;
+        if (hi == q) s += wh;
+      }
+    }
+    a[p] = s;
+    any |= s != 0.f;
+  }
+  return any;
+}
+
+// [first, last] pixel an axis' samples touch (last < 0: none)
+__device__ __forceinline__ void roi_axis_span(float a0, float bsz, int L, int& first, int& last) {
+  first = L;
+  last = -1;
+  for (int p = 0; p < 7; ++p)
+    for (int i = 0; i < 2; ++i) {
+      int lo, hi;
+      float wl, wh;
+      if (roi_axis_sample(a0, bsz, p, i, L, lo, hi, wl, wh)) {
+        first = min(first, lo);
+        last = max(last, hi);
+      }
+    }
+}
+
+template <int NJ>
+__global__ void __launch_bounds__(RB_T)
+roi_align_bwd_kernel(const float* __restrict__ rois, const float* __restrict__ dout, float* __restrict__ dmaps, int n, int H,
+                     int W, int C, float scale, int tiles_x) {
+  constexpr int R = 7;
+  __shared__ int list[RB_T];
+  __shared__ int wcount[RB_T / 32];
+  const int map = blockIdx.y;
+  const int ty0 = (blockIdx.x / tiles_x) * RB_TY, tx0 = (blockIdx.x % tiles_x) * RB_TX;
+  const int t = threadIdx.x, lane = t & 31, warp = t >> 5;
+  const int py = ty0 + (warp >> 1), px0 = tx0 + (warp & 1) * RB_PPW;
+  float4 acc[RB_PPW][NJ];
+#pragma unroll
+  for (int q = 0; q < RB_PPW; ++q)
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) acc[q][j] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int c0 = 0; c0 < n; c0 += RB_T) {
+    const int ri = c0 + t;
+    bool hit = false;
+    if (ri < n) {
+      const float* r = rois + (size_t)ri * 5;
+      if ((int)r[0] == map) {
+        const float x0 = r[1] * scale - 0.5f, y0 = r[2] * scale - 0.5f;
+        const float x1 = r[3] * scale - 0.5f, y1 = r[4] * scale - 0.5f;
+        const float bw = (x1 - x0) / (float)R, bh = (y1 - y0) / (float)R;
+        int yf, yl, xf, xl;
+        roi_axis_span(y0, bh, H, yf, yl);
+        roi_axis_span(x0, bw, W, xf, xl);
+        hit = yl >= 0 && xl >= 0 && yf < ty0 + RB_TY && yl >= ty0 && xf < tx0 + RB_TX && xl >= tx0;
+      }
+    }
+    const unsigned b = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) wcount[warp] = __popc(b);
+    __syncthreads();
+    int base = 0, total = 0;
+#pragma unroll
+    for (int w = 0; w < RB_T / 32; ++w) {
+      base += w < warp ? wcount[w] : 0;
+      total += wcount[w];
+    }
+    if (hit) list[base + __popc(b & ((1u << lane) - 1u))] = ri;
+    __syncthreads();
+    for (int s = 0; s < total; ++s) {
+      const int ri2 = list[s];
+      const float* r = rois + (size_t)ri2 * 5;
+      const float x0 = r[1] * scale - 0.5f, y0 = r[2] * scale - 0.5f;
+      const float x1 = r[3] * scale - 0.5f, y1 = r[4] * scale - 0.5f;
+      const float bw = (x1 - x0) / (float)R, bh = (y1 - y0) / (float)R;
+      float ay[7];
+      if (!roi_axis_weights(y0, bh, H, py, ay)) continue;        // warp-uniform
+      const float* g = dout + (size_t)ri2 * R * R * C;
+#pragma unroll
+      for (int q = 0; q < RB_PPW; ++q) {
+        float ax[7];
+        if (!roi_axis_weights(x0, bw, W, px0 + q, ax)) continue;
+        for (int ph = 0; ph < R; ++ph) {
+          if (ay[ph] == 0.f) continue;
+          for (int pw = 0; pw < R; ++pw) {
+            const float wgt = ay[ph] * ax[pw];
+            if (wgt == 0.f) continue;
+#pragma unroll
+            for (int j = 0; j < NJ; ++j) {
+              const int c = 4 * lane + 128 * j;
+              if (c < C) {
+                const float4 v = ldg4(g + (size_t)(ph * R + pw) * C + c);
+                acc[q][j].x = fmaf(wgt, v.x, acc[q][j].x); acc[q][j].y = fmaf(wgt, v.y, acc[q][j].y);
+                acc[q][j].z = fmaf(wgt, v.z, acc[q][j].z); acc[q][j].w = fmaf(wgt, v.w, acc[q][j].w);
+              }
+            }
+          }
+        }
+      }
+    }
+    __syncthreads();                                     // the list is rewritten by the next chunk
+  }
+  const float inv = 1.f / (float)(2 * 2);
+#pragma unroll
+  for (int q = 0; q < RB_PPW; ++q) {
+    const int px = px0 + q;
+    if (py >= H || px >= W) continue;
+    float* dst = dmaps + (((size_t)map * H + py) * W + px) * C;
+#pragma unroll
+    for (int j = 0; j < NJ; ++j) {
+      const int c = 4 * lane + 128 * j;
+      if (c < C)
+        *reinterpret_cast<float4*>(dst + c) = make_float4(acc[q][j].x * inv, acc[q][j].y * inv, acc[q][j].z * inv, acc[q][j].w * inv);
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------
 // DynamicConv core (decoder_utils.py:610-624), hidden = dim_dynamic = 128, 49 RoI bins:
 //   f1 = relu(LN1(F @ P1)); f2 = relu(LN2(f1 @ P2)); out = f2 flattened [49*128].  One CTA per query.
 // ------------------------------------------------------------------------------------------------
 constexpr int DC = 128, DR = 49;
 
 constexpr int DYN_T = 512;       // 16 warps: rows ty, ty + 16, ... per thread (the product loop is latency-bound at 8 warps)
+constexpr int DYN_NW = DYN_T / 32;
+constexpr int DYN_NR = (DR + DYN_NW - 1) / DYN_NW;      // 4
+
+// acc[i] = X[ty + 16 i][:] . Pm[:][4 tx .. 4 tx + 3] (Pm [c][d] in shared memory), the product loop of dynconv_kernel and of
+// the recompute in dynconv_bwd_kernel: one accumulation order over c, so both see the same LayerNorm inputs.
+// register tile: thread = 4 output columns (4 tx .. 4 tx + 3) x the rows ty, ty + 16, ... (4 rows); per 4 input channels
+// 4 parameter loads (float4) and 4 broadcast activation loads feed 64 FMAs (the one-column mapping spent one
+// 16-byte shared-memory load per 4 FMAs and was bound by the shared-memory pipe).
+__device__ __forceinline__ void dyn_rows_times(const float (*X)[DC], const float* Pm, float4 (&acc)[DYN_NR], int tx, int ty) {
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 2
+  for (int c = 0; c < DC; c += 4) {
+    const float4 p0 = *reinterpret_cast<const float4*>(Pm + (c + 0) * DC + 4 * tx), p1 = *reinterpret_cast<const float4*>(Pm + (c + 1) * DC + 4 * tx);
+    const float4 p2 = *reinterpret_cast<const float4*>(Pm + (c + 2) * DC + 4 * tx), p3 = *reinterpret_cast<const float4*>(Pm + (c + 3) * DC + 4 * tx);
+#pragma unroll
+    for (int i = 0; i < DYN_NR; ++i) {
+      const int r = ty + DYN_NW * i;
+      if (r < DR) {
+        const float4 x = *reinterpret_cast<const float4*>(&X[r][c]);
+        acc[i].x = fmaf(x.x, p0.x, acc[i].x); acc[i].y = fmaf(x.x, p0.y, acc[i].y);
+        acc[i].z = fmaf(x.x, p0.z, acc[i].z); acc[i].w = fmaf(x.x, p0.w, acc[i].w);
+        acc[i].x = fmaf(x.y, p1.x, acc[i].x); acc[i].y = fmaf(x.y, p1.y, acc[i].y);
+        acc[i].z = fmaf(x.y, p1.z, acc[i].z); acc[i].w = fmaf(x.y, p1.w, acc[i].w);
+        acc[i].x = fmaf(x.z, p2.x, acc[i].x); acc[i].y = fmaf(x.z, p2.y, acc[i].y);
+        acc[i].z = fmaf(x.z, p2.z, acc[i].z); acc[i].w = fmaf(x.z, p2.w, acc[i].w);
+        acc[i].x = fmaf(x.w, p3.x, acc[i].x); acc[i].y = fmaf(x.w, p3.y, acc[i].y);
+        acc[i].z = fmaf(x.w, p3.z, acc[i].z); acc[i].w = fmaf(x.w, p3.w, acc[i].w);
+      }
+    }
+  }
+}
+
 __global__ void __launch_bounds__(DYN_T)
 dynconv_kernel(const float* __restrict__ roi, const float* __restrict__ params, const float* __restrict__ g1,
                const float* __restrict__ b1, const float* __restrict__ g2, const float* __restrict__ b2,
@@ -1098,12 +1285,7 @@ dynconv_kernel(const float* __restrict__ roi, const float* __restrict__ params, 
     reinterpret_cast<float4*>(&F[0][0])[i] = ldg4(src + i * 4);
   asm volatile("cp.async.wait_group 1;" ::: "memory");
   __syncthreads();
-  // register tile: thread = 4 output columns (4 tx .. 4 tx + 3) x the rows ty, ty + 16, ... (4 rows); per 4 input channels
-  // 4 parameter loads (float4) and 4 broadcast activation loads feed 64 FMAs (the one-column mapping spent one
-  // 16-byte shared-memory load per 4 FMAs and was bound by the shared-memory pipe).  Accumulation order over c unchanged.
   const int tx = t & 31, ty = t >> 5;
-  constexpr int NW = DYN_T / 32;
-  constexpr int NR = (DR + NW - 1) / NW;      // 4
   for (int layer = 0; layer < 2; ++layer) {
     if (layer == 1) {
       asm volatile("cp.async.wait_group 0;" ::: "memory");
@@ -1111,34 +1293,13 @@ dynconv_kernel(const float* __restrict__ roi, const float* __restrict__ params, 
     }
     const float* Pm = PS + layer * DC * DC;               // [c][d] in shared memory
     float(*X)[DC] = layer == 0 ? F : T;
-    float4 acc[NR];
-#pragma unroll
-    for (int i = 0; i < NR; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-#pragma unroll 2
-    for (int c = 0; c < DC; c += 4) {
-      const float4 p0 = *reinterpret_cast<const float4*>(Pm + (c + 0) * DC + 4 * tx), p1 = *reinterpret_cast<const float4*>(Pm + (c + 1) * DC + 4 * tx);
-      const float4 p2 = *reinterpret_cast<const float4*>(Pm + (c + 2) * DC + 4 * tx), p3 = *reinterpret_cast<const float4*>(Pm + (c + 3) * DC + 4 * tx);
-#pragma unroll
-      for (int i = 0; i < NR; ++i) {
-        const int r = ty + NW * i;
-        if (r < DR) {
-          const float4 x = *reinterpret_cast<const float4*>(&X[r][c]);
-          acc[i].x = fmaf(x.x, p0.x, acc[i].x); acc[i].y = fmaf(x.x, p0.y, acc[i].y);
-          acc[i].z = fmaf(x.x, p0.z, acc[i].z); acc[i].w = fmaf(x.x, p0.w, acc[i].w);
-          acc[i].x = fmaf(x.y, p1.x, acc[i].x); acc[i].y = fmaf(x.y, p1.y, acc[i].y);
-          acc[i].z = fmaf(x.y, p1.z, acc[i].z); acc[i].w = fmaf(x.y, p1.w, acc[i].w);
-          acc[i].x = fmaf(x.z, p2.x, acc[i].x); acc[i].y = fmaf(x.z, p2.y, acc[i].y);
-          acc[i].z = fmaf(x.z, p2.z, acc[i].z); acc[i].w = fmaf(x.z, p2.w, acc[i].w);
-          acc[i].x = fmaf(x.w, p3.x, acc[i].x); acc[i].y = fmaf(x.w, p3.y, acc[i].y);
-          acc[i].z = fmaf(x.w, p3.z, acc[i].z); acc[i].w = fmaf(x.w, p3.w, acc[i].w);
-        }
-      }
-    }
+    float4 acc[DYN_NR];
+    dyn_rows_times(X, Pm, acc, tx, ty);
     __syncthreads();  // everyone finished reading X before it may be overwritten
     float(*Y)[DC] = layer == 0 ? T : F;
 #pragma unroll
-    for (int i = 0; i < NR; ++i) {
-      const int r = ty + NW * i;
+    for (int i = 0; i < DYN_NR; ++i) {
+      const int r = ty + DYN_NW * i;
       if (r < DR) *reinterpret_cast<float4*>(&Y[r][4 * tx]) = acc[i];
     }
     __syncthreads();
@@ -1166,6 +1327,203 @@ dynconv_kernel(const float* __restrict__ roi, const float* __restrict__ params, 
   float* dst = out + (size_t)qn * DR * DC;
   for (int i = t; i < DR * DC / 4; i += blockDim.x)
     *reinterpret_cast<float4*>(dst + i * 4) = reinterpret_cast<const float4*>(&F[0][0])[i];
+}
+
+// ------------------------------------------------------------------------------------------------
+// DynamicConv backward.  One CTA per query; the forward is recomputed in shared memory with dyn_rows_times and the
+// forward's LayerNorm statistics code, so Z1, Z2 and the statistics equal the forward's bit for bit.  Per query:
+//   dA2 = dY2 * [Y2 > 0]; LN2 backward -> dZ2 (in place of x^2); dP2 = Y1^T dZ2; dY1 = dZ2 P2^T;
+//   dA1 = dY1 * [Y1 > 0]; LN1 backward -> dZ1 (in place of dY1); dP1 = F^T dZ1; dF = dZ1 P1^T.
+// Shared memory: P1, P2 (128 KB) and four 49 x 128 tiles F, x^1, Y1 (then dY1, dZ1), x^2 (then dZ2): 231 424 B.
+// LayerNorm parameter gradients: per query partials (one thread per column, rows in ascending order), reduced by the
+// caller in a fixed order.  Every output element is written once: no atomics, deterministic.
+// ------------------------------------------------------------------------------------------------
+// out[c][d] = sum_r A[r][c] B[r][d] (128 x 128, to global memory): thread = columns 4 tx .. 4 tx + 3 of the rows
+// c = ty + 16 i (B loads are float4 rows, A loads warp broadcasts)
+__device__ __forceinline__ void dyn_at_b(const float (*A)[DC], const float (*Bm)[DC], float* __restrict__ out, int tx, int ty) {
+  constexpr int NC = DC / DYN_NW;      // 8
+  float4 acc[NC];
+#pragma unroll
+  for (int i = 0; i < NC; ++i) acc[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int r = 0; r < DR; ++r) {
+    const float4 bv = *reinterpret_cast<const float4*>(&Bm[r][4 * tx]);
+#pragma unroll
+    for (int i = 0; i < NC; ++i) {
+      const float a = A[r][ty + DYN_NW * i];
+      acc[i].x = fmaf(a, bv.x, acc[i].x); acc[i].y = fmaf(a, bv.y, acc[i].y);
+      acc[i].z = fmaf(a, bv.z, acc[i].z); acc[i].w = fmaf(a, bv.w, acc[i].w);
+    }
+  }
+#pragma unroll
+  for (int i = 0; i < NC; ++i) *reinterpret_cast<float4*>(out + (size_t)(ty + DYN_NW * i) * DC + 4 * tx) = acc[i];
+}
+
+// acc[i][j] = X[ty + 16 i][:] . Pm[tx + 32 j][:] (rows times Pm transposed).  Lane tx starts its walk over d at 4 tx, so the
+// 16-byte loads of one quarter-warp cover all 32 banks (rows of X and of Pm are 128 floats apart).
+__device__ __forceinline__ void dyn_rows_times_t(const float (*X)[DC], const float* Pm, float (&acc)[DYN_NR][4], int tx, int ty) {
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) acc[i][j] = 0.f;
+  for (int k = 0; k < DC / 4; ++k) {
+    const int d = ((k + tx) & (DC / 4 - 1)) * 4;
+    float4 p[4];
+#pragma unroll
+    for (int j = 0; j < 4; ++j) p[j] = *reinterpret_cast<const float4*>(Pm + (tx + 32 * j) * DC + d);
+#pragma unroll
+    for (int i = 0; i < DYN_NR; ++i) {
+      const int r = ty + DYN_NW * i;
+      if (r < DR) {
+        const float4 x = *reinterpret_cast<const float4*>(&X[r][d]);
+#pragma unroll
+        for (int j = 0; j < 4; ++j)
+          acc[i][j] = fmaf(x.w, p[j].w, fmaf(x.z, p[j].z, fmaf(x.y, p[j].y, fmaf(x.x, p[j].x, acc[i][j]))));
+      }
+    }
+  }
+}
+
+// Z (in place) -> x^ = (Z - mean) rstd with the forward's statistics code; Y = relu(x^ g + b) (Y may be null)
+__device__ __forceinline__ void dyn_ln_fwd_rows(float (*Z)[DC], float (*Y)[DC], const float* __restrict__ g,
+                                                const float* __restrict__ b, float* rstd_out, float eps, int t) {
+  for (int r = t >> 5; r < DR; r += DYN_NW) {
+    const int lane = t & 31;
+    float4 x = *reinterpret_cast<const float4*>(&Z[r][lane * 4]);
+    float mean = warp_sum(x.x + x.y + x.z + x.w) / (float)DC;
+    float dx0 = x.x - mean, dx1 = x.y - mean, dx2 = x.z - mean, dx3 = x.w - mean;
+    float var = warp_sum(dx0 * dx0 + dx1 * dx1 + dx2 * dx2 + dx3 * dx3) / (float)DC;
+    float rstd = 1.f / sqrtf(var + eps);
+    const float4 xh = make_float4(dx0 * rstd, dx1 * rstd, dx2 * rstd, dx3 * rstd);
+    *reinterpret_cast<float4*>(&Z[r][lane * 4]) = xh;
+    if (Y) {
+      const float4 gg = ldg4(g + lane * 4), be = ldg4(b + lane * 4);
+      *reinterpret_cast<float4*>(&Y[r][lane * 4]) = make_float4(fmaxf(xh.x * gg.x + be.x, 0.f), fmaxf(xh.y * gg.y + be.y, 0.f),
+                                                                fmaxf(xh.z * gg.z + be.z, 0.f), fmaxf(xh.w * gg.w + be.w, 0.f));
+    }
+    if (lane == 0) rstd_out[r] = rstd;
+  }
+}
+
+// per-query dgamma / dbeta of relu(LN(.)): thread c < 128 sums dA x^ and dA over the rows in ascending order
+__device__ __forceinline__ void dyn_ln_col(const float* dy, const float (*Xh)[DC], const float* __restrict__ g,
+                                           const float* __restrict__ b, float* out_g, float* out_b, int t) {
+  if (t >= DC) return;
+  const float gc = __ldg(g + t), bc = __ldg(b + t);
+  float sg = 0.f, sb = 0.f;
+  for (int r = 0; r < DR; ++r) {
+    const float xh = Xh[r][t];
+    const float da = xh * gc + bc > 0.f ? dy[r * DC + t] : 0.f;
+    sg = fmaf(da, xh, sg);
+    sb += da;
+  }
+  out_g[t] = sg;
+  out_b[t] = sb;
+}
+
+// dZ = rstd (dx^ - mean(dx^) - x^ mean(dx^ x^)), dx^ = dA g, dA = dY [x^ g + b > 0]; one warp per row, dZ may alias dY
+__device__ __forceinline__ void dyn_ln_bwd_rows(const float* dy, const float (*Xh)[DC], float (*Dz)[DC], const float* __restrict__ g,
+                                                const float* __restrict__ b, const float* rstd, int t) {
+  const int lane = t & 31;
+  const float4 gg = ldg4(g + lane * 4), be = ldg4(b + lane * 4);
+  for (int r = t >> 5; r < DR; r += DYN_NW) {
+    const float4 d = *reinterpret_cast<const float4*>(dy + r * DC + lane * 4);
+    const float4 x = *reinterpret_cast<const float4*>(&Xh[r][lane * 4]);
+    const float h0 = (x.x * gg.x + be.x > 0.f ? d.x : 0.f) * gg.x, h1 = (x.y * gg.y + be.y > 0.f ? d.y : 0.f) * gg.y;
+    const float h2 = (x.z * gg.z + be.z > 0.f ? d.z : 0.f) * gg.z, h3 = (x.w * gg.w + be.w > 0.f ? d.w : 0.f) * gg.w;
+    const float s1 = warp_sum(h0 + h1 + h2 + h3) / (float)DC;
+    const float s2 = warp_sum(h0 * x.x + h1 * x.y + h2 * x.z + h3 * x.w) / (float)DC;
+    const float rs = rstd[r];
+    *reinterpret_cast<float4*>(&Dz[r][lane * 4]) = make_float4((h0 - s1 - x.x * s2) * rs, (h1 - s1 - x.y * s2) * rs,
+                                                               (h2 - s1 - x.z * s2) * rs, (h3 - s1 - x.w * s2) * rs);
+  }
+}
+
+constexpr int DYN_BWD_SMEM = (2 * DC * DC + 4 * DR * DC) * (int)sizeof(float);    // 231 424 B
+
+__global__ void __launch_bounds__(DYN_T)
+dynconv_bwd_kernel(const float* __restrict__ roi, const float* __restrict__ params, const float* __restrict__ g1,
+                   const float* __restrict__ b1, const float* __restrict__ g2, const float* __restrict__ b2,
+                   const float* __restrict__ dout, float* __restrict__ droi, float* __restrict__ dparams,
+                   float* __restrict__ dnorm, float eps) {
+  extern __shared__ __align__(16) float dyn_smem[];
+  __shared__ float rstd[2][DR];
+  float* PS = dyn_smem;                                                          // P1 | P2, [c][d]
+  float(*F)[DC] = reinterpret_cast<float(*)[DC]>(dyn_smem + 2 * DC * DC);
+  float(*X1)[DC] = F + DR;              // x^1
+  float(*Y1)[DC] = F + 2 * DR;          // relu(LN1), then dY1, then dZ1
+  float(*X2)[DC] = F + 3 * DR;          // x^2, then dZ2
+  const int qn = blockIdx.x, t = threadIdx.x, tx = t & 31, ty = t >> 5;
+  {
+    const float* psrc = params + (size_t)qn * 2 * DC * DC;
+    for (int l = 0; l < 2; ++l) {
+      for (int i = t * 4; i < DC * DC; i += DYN_T * 4)
+        asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(tc::smem_u32(PS + l * DC * DC + i)), "l"(psrc + l * DC * DC + i)
+                     : "memory");
+      asm volatile("cp.async.commit_group;" ::: "memory");
+    }
+  }
+  const float* src = roi + (size_t)qn * DR * DC;
+  for (int i = t; i < DR * DC / 4; i += DYN_T) reinterpret_cast<float4*>(&F[0][0])[i] = ldg4(src + i * 4);
+  asm volatile("cp.async.wait_group 1;" ::: "memory");
+  __syncthreads();
+  // forward recompute
+  float4 acc[DYN_NR];
+  dyn_rows_times(F, PS, acc, tx, ty);
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i)
+    if (ty + DYN_NW * i < DR) *reinterpret_cast<float4*>(&X1[ty + DYN_NW * i][4 * tx]) = acc[i];
+  __syncthreads();
+  dyn_ln_fwd_rows(X1, Y1, g1, b1, rstd[0], eps, t);
+  asm volatile("cp.async.wait_group 0;" ::: "memory");
+  __syncthreads();
+  dyn_rows_times(Y1, PS + DC * DC, acc, tx, ty);
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i)
+    if (ty + DYN_NW * i < DR) *reinterpret_cast<float4*>(&X2[ty + DYN_NW * i][4 * tx]) = acc[i];
+  __syncthreads();
+  dyn_ln_fwd_rows(X2, nullptr, g2, b2, rstd[1], eps, t);
+  __syncthreads();
+  // second layer
+  const float* dy2 = dout + (size_t)qn * DR * DC;
+  float* dn = dnorm + (size_t)qn * 4 * DC;                 // dgamma1 | dbeta1 | dgamma2 | dbeta2
+  dyn_ln_col(dy2, X2, g2, b2, dn + 2 * DC, dn + 3 * DC, t);
+  __syncthreads();
+  dyn_ln_bwd_rows(dy2, X2, X2, g2, b2, rstd[1], t);
+  __syncthreads();
+  float* dp = dparams + (size_t)qn * 2 * DC * DC;
+  dyn_at_b(Y1, X2, dp + DC * DC, tx, ty);                  // dP2 = Y1^T dZ2
+  float acc2[DYN_NR][4];
+  dyn_rows_times_t(X2, PS + DC * DC, acc2, tx, ty);        // dY1 = dZ2 P2^T
+  __syncthreads();
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i)
+    if (ty + DYN_NW * i < DR)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) Y1[ty + DYN_NW * i][tx + 32 * j] = acc2[i][j];
+  __syncthreads();
+  // first layer
+  dyn_ln_col(&Y1[0][0], X1, g1, b1, dn, dn + DC, t);
+  __syncthreads();
+  dyn_ln_bwd_rows(&Y1[0][0], X1, Y1, g1, b1, rstd[0], t);
+  __syncthreads();
+  dyn_at_b(F, Y1, dp, tx, ty);                              // dP1 = F^T dZ1
+  dyn_rows_times_t(Y1, PS, acc2, tx, ty);                   // dF = dZ1 P1^T
+  float* dst = droi + (size_t)qn * DR * DC;
+#pragma unroll
+  for (int i = 0; i < DYN_NR; ++i)
+    if (ty + DYN_NW * i < DR)
+#pragma unroll
+      for (int j = 0; j < 4; ++j) dst[(ty + DYN_NW * i) * DC + tx + 32 * j] = acc2[i][j];
+}
+
+// dx = dy (Phi(h) + h phi(h)): the derivative of the exact (erf) GELU of di_gelu
+__global__ void gelu_bwd_kernel(const float* __restrict__ dy, const float* __restrict__ h, float* __restrict__ dx, long long n) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const float v = h[i];
+  const float cdf = 0.5f * (1.f + erff(v * 0.70710678118654752440f));
+  const float pdf = 0.39894228040143267794f * expf(-0.5f * v * v);
+  dx[i] = dy[i] * fmaf(v, pdf, cdf);
 }
 
 // layout converters (drop-in boundary: the reference hands NCHW tensors around)
@@ -1574,6 +1932,48 @@ int di_dynconv_f32(const float* roi, const float* params, const float* g1, const
   }
   dynconv_kernel<<<n, DYN_T, smem, stream>>>(roi, params, g1, b1, g2, b2, out, eps);
   DI_CHECK_LAUNCH("di_dynconv_f32");
+  return DI_OK;
+}
+
+// Backward of di_roi_align_f32 w.r.t. the maps: d_out [n, 49, C] -> d_maps [n_maps, H, W, C], every pixel written (0 where
+// no sample reaches); RoIs with a map index outside [0, n_maps) contribute nothing.  Deterministic (a gather, no atomics).
+int di_roi_align_bwd_f32(const float* rois, const float* d_out, float* d_maps, int n, int n_maps, int H, int W, int C,
+                         float scale, cudaStream_t stream) {
+  DI_CHECK_ARG(d_maps && (n == 0 || (rois && d_out)) && n >= 0 && n_maps > 0 && H > 0 && W > 0 && C > 0 && C % 4 == 0 &&
+                   C <= 512 && (((uintptr_t)d_out | (uintptr_t)d_maps) & 15) == 0,
+               "di_roi_align_bwd_f32: bad argument (n=%d n_maps=%d H=%d W=%d C=%d)", n, n_maps, H, W, C);
+  DI_CHECK_ARG(n_maps <= 65535, "di_roi_align_bwd_f32: n_maps <= 65535");
+  const int tiles_x = di_cdiv(W, RB_TX);
+  dim3 grid(tiles_x * di_cdiv(H, RB_TY), n_maps);
+  if (C <= 128) roi_align_bwd_kernel<1><<<grid, RB_T, 0, stream>>>(rois, d_out, d_maps, n, H, W, C, scale, tiles_x);
+  else if (C <= 256) roi_align_bwd_kernel<2><<<grid, RB_T, 0, stream>>>(rois, d_out, d_maps, n, H, W, C, scale, tiles_x);
+  else roi_align_bwd_kernel<4><<<grid, RB_T, 0, stream>>>(rois, d_out, d_maps, n, H, W, C, scale, tiles_x);
+  DI_CHECK_LAUNCH("di_roi_align_bwd_f32");
+  return DI_OK;
+}
+
+// Backward of di_dynconv_f32: d_out [n, 49*128] -> d_roi [n, 49, 128], d_params [n, 2*128*128] (layout of params),
+// d_norm [n, 4*128] = per-query partials of dgamma1 | dbeta1 | dgamma2 | dbeta2 (sum over n with di_col_sum_f32).
+int di_dynconv_bwd_f32(const float* roi, const float* params, const float* g1, const float* b1, const float* g2, const float* b2,
+                       const float* d_out, float* d_roi, float* d_params, float* d_norm, int n, float eps, cudaStream_t stream) {
+  DI_CHECK_ARG(roi && params && g1 && b1 && g2 && b2 && d_out && d_roi && d_params && d_norm && n > 0 &&
+                   (((uintptr_t)params | (uintptr_t)roi | (uintptr_t)d_out | (uintptr_t)d_params | (uintptr_t)g1 |
+                     (uintptr_t)b1 | (uintptr_t)g2 | (uintptr_t)b2) & 15) == 0,
+               "di_dynconv_bwd_f32: bad argument");
+  static DiSmemOnce once{};
+  if (!di_smem_once(once, dynconv_bwd_kernel, DYN_BWD_SMEM)) {
+    di_set_error("di_dynconv_bwd_f32: cannot reserve shared memory");
+    return DI_ERR_LAUNCH;
+  }
+  dynconv_bwd_kernel<<<n, DYN_T, DYN_BWD_SMEM, stream>>>(roi, params, g1, b1, g2, b2, d_out, d_roi, d_params, d_norm, eps);
+  DI_CHECK_LAUNCH("di_dynconv_bwd_f32");
+  return DI_OK;
+}
+
+int di_gelu_bwd_f32(const float* dy, const float* h, float* dx, long long n, cudaStream_t stream) {
+  DI_CHECK_ARG(dy && h && dx && n > 0, "di_gelu_bwd_f32: bad argument");
+  gelu_bwd_kernel<<<di_cdiv(n, 256), 256, 0, stream>>>(dy, h, dx, n);
+  DI_CHECK_LAUNCH("di_gelu_bwd_f32");
   return DI_OK;
 }
 

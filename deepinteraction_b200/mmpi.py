@@ -477,43 +477,13 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
             # RoI reads <= one map; DynamicConv parameter generator weights 128 x 32768 (+ out_layer 6272 x 128) read once
             ops._MODULE[0] = ('ImageRCNNBlock' if bp['image'] else 'PointRCNNBlock',
                               4 * (B * P * 49 * C) + 4 * (C * 2 * C * C + 49 * C * C), 2 * B * P * (C * 2 * C * C + 2 * 49 * C * C + 49 * C * C))
-            if bp['image']:
-                rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 0, prm, proj, aux)
-                roi = ops.roi_align(img, rois, 1.0 / self.out_size_factor_img)
-            else:
-                rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 1, prm)
-                roi = ops.roi_align(new_pts, rois, 1.0)
-            w, b, wo, bo = bp['attn']
-            qkv = self._mlp([prev], w, b)
-            a = ops.mha_small(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H, onbits, win)
-            q1 = self._mlp([a], wo, bo, res=prev, ln=bp['norm1'])
-            ops.TC_BF16[0] = _DYN_BF16                       # parameter generator (M=P, N=32768): see _DYN_BF16
-            params = ops.linear([q1], *bp['dyn'])
-            ops.TC_BF16[0] = False
-            flat = ops.dynconv(roi, params, *bp['dn1'], *bp['dn2'])
-            part = ops.linear([flat], bp['dout'][0], splits=49)
-            t = ops.rows_finish(part, bias=bp['dout'][1], gamma=bp['dn3'][0], beta=bp['dn3'][1], act=ops.ACT_RELU)
-            q2 = ops.rows_finish(t, res=q1, gamma=bp['norm2'][0], beta=bp['norm2'][1])
-            f1w, f1b, f2w, f2b = bp['ffn']
+            q, rois, win = self._rcnn_block(bp, prev, pred, new_pts, img, B, P, prm, proj, aux)
             if bp['v2']:
-                # decoder_utils.py:971-988 / :1071-1085.  The self branch every query of a (sample, view) group receives
-                # is the one of the group's FIRST query (the reference's (1,n,C) + (n,1,C) broadcast followed by [0];
-                # oracle/mmpi_pp.py), so it is evaluated on the B*V "leader" rows only.
-                q3 = self._mlp([q2], f1w, f1b, ops.ACT_RELU, f2w, f2b, res=q2, ln=bp['norm3'])
-                Vg = V if bp['image'] else 1
-                lrow, lwin = ops.rcnn_leaders(onbits, B, P, Vg)
-                a_l = ops.mha_small_rows(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H, onbits, lrow, lwin)
-                q1_l = self._mlp([a_l], wo, bo, res=ops.take_rows(prev, lrow), ln=bp['norm1'])
-                s1w, s1b, s2w, s2b = bp['self_ffn']
-                s_l = self._mlp([q1_l], s1w, s1b, ops.ACT_RELU, s2w, s2b, res=q1_l, ln=bp['self_norm'])
-                q = ops.branch_mix(q3, s_l, win, bp['scale'], bp['self_scale'], P, Vg, bp['image'])
                 ops._MODULE[0] = ('prediction_heads', 0, 0)
                 pred = self._pred(bp['pred'], [q])
                 ops.pred_finish_pp(pred, qpos, look, first, win if bp['image'] else None, keep, li == 0)
                 keeps.append(keep.clone())
             else:
-                q = self._mlp([q2], f1w, f1b, ops.ACT_GELU, f2w, f2b, res=q2, ln=bp['norm3'],
-                              zero_if_neg=win if bp['image'] else None)
                 ops._MODULE[0] = ('prediction_heads', 0, 0)
                 pred = self._pred(bp['pred'], [q, prev])
                 ops.pred_finish(pred, qpos, first if bp['image'] else None, win if bp['image'] else None)
@@ -560,6 +530,54 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
                          z2=self._mlp([a2], *pk['cross_out'], res=q1), q2=q2, f=f, z3=self._mlp([f], f2w, f2b, res=q2),
                          kk=ops.add_rows_mod(bev.reshape(B * HW, C), pk['cross_pe']['kpe']))
         return q3
+
+    def _rcnn_block(self, bp, prev, pred, new_pts, img, B, P, prm, proj, aux, saved=None):
+        """One RCNN block of the MMPI layers (decoder_utils.py:632-1089) on query rows: prev [B*P, C], pred [B*P, NP] (the
+        previous layer's predictions, which give the RoIs), new_pts [B, Y, X, C] (BEV blocks) or img [B*V, h, w, C] (image
+        blocks) -> (rows [B*P, C], rois [B*P, 5], win [B*P]).  The one implementation of the block, for the forward
+        schedule and for the eager re-run of backward.point_rcnn_backward; saved (a dict, V1 blocks) additionally stores
+        the values the backward needs, with the returned rows unchanged."""
+        C, H, V = self.hidden_channel, self.num_heads, self.num_views
+        if bp['image']:
+            rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 0, prm, proj, aux)
+            roi = ops.roi_align(img, rois, 1.0 / self.out_size_factor_img)
+        else:
+            rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 1, prm)
+            roi = ops.roi_align(new_pts, rois, 1.0)
+        w, b, wo, bo = bp['attn']
+        qkv = self._mlp([prev], w, b)
+        a = ops.mha_small(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H, onbits, win)
+        q1 = self._mlp([a], wo, bo, res=prev, ln=bp['norm1'])
+        ops.TC_BF16[0] = _DYN_BF16                       # parameter generator (M=P, N=32768): see _DYN_BF16
+        params = ops.linear([q1], *bp['dyn'])
+        ops.TC_BF16[0] = False
+        flat = ops.dynconv(roi, params, *bp['dn1'], *bp['dn2'])
+        part = ops.linear([flat], bp['dout'][0], splits=49)
+        t = ops.rows_finish(part, bias=bp['dout'][1], gamma=bp['dn3'][0], beta=bp['dn3'][1], act=ops.ACT_RELU)
+        q2 = ops.rows_finish(t, res=q1, gamma=bp['norm2'][0], beta=bp['norm2'][1])
+        f1w, f1b, f2w, f2b = bp['ffn']
+        if bp['v2']:
+            # decoder_utils.py:971-988 / :1071-1085.  The self branch every query of a (sample, view) group receives
+            # is the one of the group's FIRST query (the reference's (1,n,C) + (n,1,C) broadcast followed by [0];
+            # oracle/mmpi_pp.py), so it is evaluated on the B*V "leader" rows only.
+            q3 = self._mlp([q2], f1w, f1b, ops.ACT_RELU, f2w, f2b, res=q2, ln=bp['norm3'])
+            Vg = V if bp['image'] else 1
+            lrow, lwin = ops.rcnn_leaders(onbits, B, P, Vg)
+            a_l = ops.mha_small_rows(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], B, P, H, onbits, lrow, lwin)
+            q1_l = self._mlp([a_l], wo, bo, res=ops.take_rows(prev, lrow), ln=bp['norm1'])
+            s1w, s1b, s2w, s2b = bp['self_ffn']
+            s_l = self._mlp([q1_l], s1w, s1b, ops.ACT_RELU, s2w, s2b, res=q1_l, ln=bp['self_norm'])
+            return ops.branch_mix(q3, s_l, win, bp['scale'], bp['self_scale'], P, Vg, bp['image']), rois, win
+        q = self._mlp([q2], f1w, f1b, ops.ACT_GELU, f2w, f2b, res=q2, ln=bp['norm3'],
+                      zero_if_neg=win if bp['image'] else None)
+        if saved is not None:
+            # pre-norm sums and the FFN's hidden rows, which the fused row kernels do not return
+            h = self._mlp([q2], f1w, f1b)
+            f = self._mlp([q2], f1w, f1b, ops.ACT_GELU)
+            saved.update(rois=rois, qkv=qkv, a=a, z1=self._mlp([a], wo, bo, res=prev), q1=q1, params=params, roi=roi,
+                         flat=flat, part=part, zd3=ops.rows_finish(part, bias=bp['dout'][1]), t=t,
+                         z2=ops.rows_finish(t, res=q1), q2=q2, h=h, f=f, z3=self._mlp([f], f2w, f2b, res=q2))
+        return q, rois, win
 
     def _to_dict(self, pred, B, P):
         t = pred.view(B, P, self.NP).permute(0, 2, 1)

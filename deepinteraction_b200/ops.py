@@ -619,6 +619,39 @@ def dynconv(roi, params, g1, b1, g2, b2, eps=1e-5):
     return out
 
 
+def roi_align_bwd(d_out, rois, n_maps, H, W, scale):
+    """Gradient of roi_align w.r.t. the maps: d_out [n, 49, C] -> d_maps [n_maps, H, W, C] (every pixel written)."""
+    n, _, C = d_out.shape
+    assert d_out.is_contiguous() and rois.is_contiguous() and d_out.shape[1] == 49 and rois.shape == (n, 5)
+    d_maps = torch.empty(n_maps, H, W, C, device=d_out.device, dtype=torch.float32)
+    _call('di_roi_align_bwd_f32', _ptr(rois), _ptr(d_out), _ptr(d_maps), n, n_maps, H, W, C, float(scale), _stream(),
+          nbytes=4 * (d_out.numel() + d_maps.numel()))
+    return d_maps
+
+
+def dynconv_bwd(roi, params, g1, b1, g2, b2, d_out, eps=1e-5):
+    """Gradient of dynconv: -> (d_roi [n, 49, 128], d_params [n, 32768], d_norm [n, 512] per-query partials of
+    dgamma1 | dbeta1 | dgamma2 | dbeta2)."""
+    n = roi.shape[0]
+    assert roi.shape[1:] == (49, 128) and params.shape == (n, 2 * 128 * 128) and d_out.shape == (n, 49 * 128)
+    assert roi.is_contiguous() and params.is_contiguous() and d_out.is_contiguous()
+    d_roi = torch.empty(n, 49, 128, device=roi.device, dtype=torch.float32)
+    d_params = torch.empty(n, 2 * 128 * 128, device=roi.device, dtype=torch.float32)
+    d_norm = torch.empty(n, 4 * 128, device=roi.device, dtype=torch.float32)
+    _call('di_dynconv_bwd_f32', _ptr(roi), _ptr(params), _ptr(g1), _ptr(b1), _ptr(g2), _ptr(b2), _ptr(d_out), _ptr(d_roi),
+          _ptr(d_params), _ptr(d_norm), n, float(eps), _stream(),
+          nbytes=4 * (2 * roi.numel() + 2 * params.numel() + d_out.numel() + d_norm.numel()),
+          flops=6 * 2 * 2 * n * 49 * 128 * 128)
+    return d_roi, d_params, d_norm
+
+
+def gelu_bwd(dy, h):
+    assert dy.is_contiguous() and h.is_contiguous() and dy.shape == h.shape
+    dx = torch.empty_like(dy)
+    _call('di_gelu_bwd_f32', _ptr(dy), _ptr(h), _ptr(dx), dy.numel(), _stream(), nbytes=12 * dy.numel())
+    return dx
+
+
 def nchw_to_nhwc(x):
     N, C, H, W = x.shape
     assert x.is_contiguous()

@@ -436,6 +436,24 @@ int di_xattn_bwd_f32(const void* q, const void* k, const void* v, const float* o
                      const float* lse, float* work, float* dq, float* dk, float* dv, int ld_dkv, int B, int P, int HW,
                      int heads, cudaStream_t stream);
 
+/* ---- backward of the RCNN blocks' kernels (decoder.cu; host composition: backward.py point_rcnn_backward)
+ * di_roi_align_bwd_f32: gradient of di_roi_align_f32 w.r.t. the maps.  rois [n, 5] and scale as in the forward (map index < 0
+ * or >= n_maps: no contribution), d_out [n, 49, C] -> d_maps [n_maps, H, W, C], every pixel written (exactly 0 where no
+ * sample reaches: no memset needed).  Same skip, clamp and last-pixel rules as the forward.  A gather over pixel tiles,
+ * RoIs summed in ascending index: deterministic, no atomics, no workspace.  n >= 0, C % 4 == 0, C <= 512, d_out and d_maps
+ * 16-byte aligned.
+ * di_dynconv_bwd_f32: gradient of di_dynconv_f32.  roi [n, 49, 128], params [n, 2*128*128], g1, b1, g2, b2 [128], d_out
+ * [n, 49*128] -> d_roi [n, 49, 128], d_params [n, 2*128*128] (P1 then P2, [c][d], as params), d_norm [n, 4*128] = per-query
+ * partials of dgamma1 | dbeta1 | dgamma2 | dbeta2 (reduce over n with di_col_sum_f32).  One CTA per query recomputes the
+ * forward in shared memory (231 424 B of dynamic shared memory); no workspace, deterministic, no atomics.  roi, params,
+ * d_out, d_params and the norm vectors 16-byte aligned.
+ * di_gelu_bwd_f32: dx = dy (Phi(h) + h phi(h)), the derivative of the exact (erf) GELU at the pre-activation h; n elements. */
+int di_roi_align_bwd_f32(const float* rois, const float* d_out, float* d_maps, int n, int n_maps, int H, int W, int C,
+                         float scale, cudaStream_t stream);
+int di_dynconv_bwd_f32(const float* roi, const float* params, const float* g1, const float* b1, const float* g2, const float* b2,
+                       const float* d_out, float* d_roi, float* d_params, float* d_norm, int n, float eps, cudaStream_t stream);
+int di_gelu_bwd_f32(const float* dy, const float* h, float* dx, long long n, cudaStream_t stream);
+
 #ifdef __cplusplus
 }
 #endif
