@@ -11,34 +11,49 @@ eps)), and d beta = d bias_folded.  Train-mode BatchNorm (batch statistics with 
 covered.  The intermediates are recomputed in fp32 (q1, k1, q, k, v and the [P, 81] attention weights), the window
 products run in the unfused kernels of csrc/lcab_bwd.cu, dense products on the wgmma / FFMA GEMMs.
 """
+import contextlib
+
 import torch
 
 from . import fold, ops
 
 
-class _precise:
+@contextlib.contextmanager
+def _precise():
     """Gradient products run on the 3xTF32 split (error ~1e-7 per product) rather than the bf16 split of the inference
-    path (~1e-5): the backward chains a dozen products per layer."""
+    path (~1e-5): the backward chains a dozen products per layer.  A context manager and a decorator; it nests (each use
+    restores the mode it found) and restores the mode when the body raises."""
+    saved, ops.TC_BF16[0] = ops.TC_BF16[0], False
+    try:
+        yield
+    finally:
+        ops.TC_BF16[0] = saved
 
-    def __enter__(self):
-        self.saved = ops.TC_BF16[0]
-        ops.TC_BF16[0] = False
 
-    def __exit__(self, *a):
-        ops.TC_BF16[0] = self.saved
+def _transposed(w):
+    """Weight [N, K] on the device (a fold.Weight or a tensor of any float type) -> fold.Weight [K, N] of the dX product
+    dx = dy W, its splits built on first use."""
+    w = getattr(w, 'w', w).detach()
+    return fold.Weight(w.t().contiguous(), w.device, lazy=True)
+
+
+_ONE = {}
+
+
+def _add(a, b):
+    """a + b on the device; None stands for zero."""
+    if a is None or b is None:
+        return b if a is None else a
+    if a.device not in _ONE:
+        _ONE[a.device] = torch.ones(1, device=a.device)
+    return ops.axpy(a.contiguous(), b.contiguous(), _ONE[a.device])
 
 
 def _bw_pack(pk):
     """Transposed weights for the dX products, built once per pack."""
-    if '_bw' in pk:
-        return pk['_bw']
-    C = pk['C']
-    dev = pk['b_self'].device
-    w1, w2 = pk['w_self'].w.detach().cpu().double(), pk['w_2'].w.detach().cpu().double()
-    wq1, wk1, wv = w1[:C], w1[C:2 * C], w1[2 * C:]
-    wq2, wk2 = w2[:C], w2[C:]
-    T = lambda m: fold.Weight(m.t().contiguous(), dev)
-    pk['_bw'] = dict(q2=T(wq2), k2=T(wk2), q1=T(wq1), kv1=T(torch.cat([wk1, wv], 0)), self1=T(torch.cat([wq1, wk1, wv], 0)))
+    if '_bw' not in pk:
+        pk['_bw'] = dict(q2=_transposed(pk['w_q2']), k2=_transposed(pk['w_k2']), q1=_transposed(pk['w_q1']),
+                         kv1=_transposed(pk['w_kv1']), self1=_transposed(pk['w_self']))
     return pk['_bw']
 
 
@@ -55,17 +70,28 @@ def _wgrad(dy, x):
     return ops.rows_finish(part) if part.shape[0] > 1 else part[0]
 
 
+def _layer_grads(dy, *xs):
+    """Parameter gradients of the dense layer y = cat(xs, 1) W^T + b from its output gradient dy [M, N] and its inputs
+    [M, K_i] -> (dW [N, sum K_i], db [N])."""
+    dW = [_wgrad(dy, x.contiguous()) for x in xs]
+    return (dW[0] if len(dW) == 1 else torch.cat(dW, 1)), ops.col_sum(dy)
+
+
+def _window_backward(q, k, v, A, dO, dims, ks, scale):
+    """Backward of out = gather(A, v), A = softmax(scale * dot(q, k)) over the ks x ks windows of a dims = (N, H, W) map:
+    q / k / v / dO [N*H*W, C] rows, A [N*H*W, ks*ks] -> (dq, dk, dv)."""
+    dA = ops.win_dot(dO, v, *dims, ks)
+    dv = ops.win_scatter(A, dO, *dims, ks)
+    dS = ops.win_softmax_bwd(A, dA, scale)
+    return ops.win_gather(dS, k, *dims, ks), ops.win_scatter(dS, q, *dims, ks), dv
+
+
+@_precise()
 def lcab_backward(pk, target, source, N, H, W, grad_out):
     """target / source / grad_out: [N*H*W, C] fp32 pixel-major rows (same tensor object for target and source = self
     attention).  -> dict(d_target, d_source (None for self attention: summed into d_target), and per layer name in
     (q1, q2, k1, k2, v) a pair (dW_folded [C, C], db_folded [C]))."""
-    with _precise():
-        return _lcab_backward(pk, target, source, N, H, W, grad_out)
-
-
-def _lcab_backward(pk, target, source, N, H, W, grad_out):
     C, ks = pk['C'], pk['ks']
-    M = N * H * W
     bw = _bw_pack(pk)
     self_attn = target is source
     x_t, x_s, dO = target.contiguous(), source.contiguous(), grad_out.contiguous()
@@ -82,24 +108,19 @@ def _lcab_backward(pk, target, source, N, H, W, grad_out):
     k = ops.linear([k1], pk['w_k2'], pk['b_k2'], R)
     scale = 1.0 / float(C) ** 0.5
     A = ops.win_softmax(ops.win_dot(q, k, N, H, W, ks), scale)
-    # window attention
-    dA = ops.win_dot(dO, v, N, H, W, ks)
-    dv = ops.win_scatter(A, dO, N, H, W, ks)
-    dS = ops.win_softmax_bwd(A, dA, scale)
-    dq = ops.win_gather(dS, k, N, H, W, ks)
-    dk = ops.win_scatter(dS, q, N, H, W, ks)
+    dq, dk, dv = _window_backward(q, k, v, A, dO, (N, H, W), ks, scale)
     # projections: ReLU masks from the saved outputs, dX on the GEMM kernels, dW as split-K products, db as column sums
     g = {}
     dq = ops.relu_bwd(dq, q)
     dk = ops.relu_bwd(dk, k)
     dv = ops.relu_bwd(dv, v)
-    g['q2'] = (_wgrad(dq, q1), ops.col_sum(dq))
-    g['k2'] = (_wgrad(dk, k1), ops.col_sum(dk))
+    g['q2'] = _layer_grads(dq, q1)
+    g['k2'] = _layer_grads(dk, k1)
     dq1 = ops.relu_bwd(ops.linear([dq], bw['q2']), q1)
     dk1 = ops.relu_bwd(ops.linear([dk], bw['k2']), k1)
-    g['q1'] = (_wgrad(dq1, x_t), ops.col_sum(dq1))
-    g['k1'] = (_wgrad(dk1, x_s), ops.col_sum(dk1))
-    g['v'] = (_wgrad(dv, x_s), ops.col_sum(dv))
+    g['q1'] = _layer_grads(dq1, x_t)
+    g['k1'] = _layer_grads(dk1, x_s)
+    g['v'] = _layer_grads(dv, x_s)
     if self_attn:
         d_t, d_s = ops.linear([dq1, dk1, dv], bw['self1']), None
     else:
@@ -107,6 +128,7 @@ def _lcab_backward(pk, target, source, N, H, W, grad_out):
     return dict(d_target=d_t, d_source=d_s, **g)
 
 
+@_precise()
 def i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_out, dropout=None):
     """Backward of the MMRI_I2P block as the product evaluates it (mmri.DeepInteractionEncoder.i2p; reference
     encoder_utils.py:216-320): rows = pts[coors]; qk = M1 rows + c1; s = attend(qk, image samples); o = M2 s + c2;
@@ -114,11 +136,6 @@ def i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_o
     (fold.i2p_fold); proj: [B, V, 12] device camera rows (mmri.Geometry.proj).  grad_out [B, Y, X, C].
     -> dict(d_pts [B,Y,X,C], d_img [B*V,h,w,C], dM1, dc1, dM2, dc2); fold.i2p_unfold_grads maps the last four to the
     attention module's own parameters.  dropout = (p, seed): the training-mode attention dropout the forward used."""
-    with _precise():
-        return _i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_out, dropout)
-
-
-def _i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_out, dropout=None):
     M1, c1, M2, c2 = i2p_pack
     coors = pts_metas['pillar_coors']
     pillars, npts = pts_metas['pillars'], pts_metas['pillars_num_points']
@@ -129,35 +146,21 @@ def _i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_
         return dict(d_pts=d_pts, d_img=d_img, dM1=z(M1), dc1=z(c1), dM2=z(M2), dc2=z(c2))
     dev = pts_nhwc.device
     # a plain tensor (the [C, C + 4] output weight of the dropout form) stays on the FFMA path
-    T_ = lambda Wt: (fold.Weight(Wt.w.detach().t().contiguous(), dev, lazy=True) if hasattr(Wt, 'w') else Wt.detach().t().contiguous())
+    M2t = _transposed(M2) if hasattr(M2, 'w') else M2.detach().t().contiguous()
     # forward intermediates
     rows = ops.gather_rows(pts_nhwc, coors)
     qk = ops.linear([rows], M1, c1)
     s, cnt = ops.i2p_attend(qk, pillars, npts, coors, proj, img_nhwc, V, in_hw, dropout=dropout)
     # out = scatter(M2 s + c2) at pillars with cnt > 0
     do = ops.gather_rows_masked(grad_out.contiguous(), cnt, coors)
-    dM2, dc2 = _wgrad(do, s), ops.col_sum(do)
-    ds = ops.linear([do], T_(M2))
+    dM2, dc2 = _layer_grads(do, s)
+    ds = ops.linear([do], M2t)
     dqk = ops.i2p_attend_bwd(qk, ds, pillars, npts, coors, proj, img_nhwc, d_img, V, in_hw, dropout)
-    dM1, dc1 = _wgrad(dqk, rows), ops.col_sum(dqk)
-    drows = ops.linear([dqk], T_(M1))
+    dM1, dc1 = _layer_grads(dqk, rows)
+    drows = ops.linear([dqk], _transposed(M1))
     ones = torch.ones(coors.shape[0], device=dev, dtype=torch.int32)
     ops.scatter_rows(drows, ones, coors, d_pts)             # one pillar per BEV cell: a plain store
     return dict(d_pts=d_pts, d_img=d_img, dM1=dM1, dc1=dc1, dM2=dM2, dc2=dc2)
-
-
-def _t_weight(W, device):
-    return fold.Weight(W.w.detach().t().contiguous(), device, lazy=True)
-
-
-def _conv3x3_transposed(w_packed, cin, device):
-    """Packed forward weight [Cout, (ky*3+kx)*Cin + ci] -> packed weight of the input-gradient convolution
-    [Cin, (ky*3+kx)*Cout + co] with the taps flipped (d x = conv3x3(d y, W^T flipped))."""
-    w = w_packed.w.detach()                                        # stays on the device: no host round trip
-    cout = w.shape[0]
-    w4 = w.view(cout, 3, 3, cin)                                   # co, ky, kx, ci
-    wt = w4.flip(1, 2).permute(3, 1, 2, 0).reshape(cin, 9 * cout)   # ci, ky', kx', co
-    return fold.Weight(wt.contiguous(), device, lazy=True)
 
 
 def conv3x3_wgrad(x_nchw, g_rows, cout):
@@ -173,6 +176,45 @@ def conv3x3_wgrad(x_nchw, g_rows, cout):
     return dw, ops.col_sum(g_rows)
 
 
+def _encoder_geometry(enc, img_feats, pts_feats, img_metas, pts_metas):
+    """Common start of the two encoder steps -> (V, pm, g): views per sample, pts_metas in the schedule's canonical form on
+    the device (with the raw points, which the geometry reads) and the frame's mmri.Geometry, finished."""
+    from . import mmri
+    dev = img_feats.device
+    (BV, _, h, w), (B, _, Y, X) = img_feats.shape, pts_feats.shape
+    pm = enc._canon_pts_metas(pts_metas, dev)
+    pm['pts'] = [p.to(dev) for p in pts_metas['pts']]
+    g = mmri.Geometry(img_metas, pm, (h, w), (Y, X), dev)
+    g.wait()
+    return BV // B, pm, g
+
+
+def _seed_rows(d_out, like):
+    """Gradient of an output map as rows [M, C] (None = zero), the shape of the map `like` [..., C]."""
+    C = like.shape[-1]
+    return d_out.reshape(-1, C).contiguous() if d_out is not None else torch.zeros(like.numel() // C, C, device=like.device)
+
+
+def _shared_conv_backward(g_rows, w_packed, x_nchw):
+    """Backward of a shared 3x3 convolution y = conv3x3(x) from d y as rows [N*H*W, Cout] -> (d x [N, H, W, Cin],
+    (dW [Cout, Cin, 3, 3], db)).  d x = conv3x3(d y, W^T flipped): the packed forward weight [Cout, (ky*3+kx)*Cin + ci]
+    becomes the packed weight [Cin, (ky*3+kx)*Cout + co] with the taps flipped, on the device."""
+    N, cin, H, W = x_nchw.shape
+    w = w_packed.w.detach()
+    cout = w.shape[0]
+    wt = w.view(cout, 3, 3, cin).flip(1, 2).permute(3, 1, 2, 0).reshape(cin, 9 * cout)   # co, ky, kx, ci -> ci, ky', kx', co
+    dx = ops.conv3x3(g_rows.view(N, H, W, cout), fold.Weight(wt.contiguous(), w.device, lazy=True), None, cout=cin, x_nhwc=True)
+    return dx, conv3x3_wgrad(x_nchw, g_rows, cout)
+
+
+def _fuse_bw_pack(lp):
+    """Transposed weights of the two fuse layers of an encoder layer pack, built once per pack."""
+    if '_bw' not in lp:
+        lp['_bw'] = dict(i_fuse=_transposed(lp['i_fuse'][0]), p_fuse=_transposed(lp['p_fuse'][0]))
+    return lp['_bw']
+
+
+@_precise()
 def encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_pts_conv, d_pts):
     """Backward of DeepInteractionEncoder.forward (base model, hidden width 128, BatchNorm in eval mode = the folded
     weights of the forward; reference deepinteraction_encoder.py:8-85).  img_feats (B*V, Ci, h, w), pts_feats
@@ -181,22 +223,11 @@ def encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_p
     -> dict(d_img_feats [B*V, h, w, Ci], d_pts_feats [B, Y, X, Cp] (pixel-major), layers = per encoder layer the folded
     parameter gradients: i2p (dM1, dc1, dM2, dc2), p_iml / p2i / i_iml (lcab_backward dicts), p_fuse / i_fuse (dW [C, 3C], db)).
     shared_conv = dict(img / pts -> (dW [C, Cin, 3, 3], db)).  The forward is re-run eagerly with its intermediates kept."""
-    with _precise():
-        return _encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_pts_conv, d_pts)
-
-
-def _encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_pts_conv, d_pts):
     from . import mmri
     pk = enc.pack()
-    dev = img_feats.device
     C = enc.hidden_channel
-    BV, Ci, h, w = img_feats.shape
-    B, Cp, Y, X = pts_feats.shape
-    V = BV // B
-    pm = enc._canon_pts_metas(pts_metas, dev)
-    pm['pts'] = [p.to(dev) for p in pts_metas['pts']]
-    g = mmri.Geometry(img_metas, pm, (h, w), (Y, X), dev)
-    g.wait()
+    (BV, _, h, w), (B, _, Y, X) = img_feats.shape, pts_feats.shape
+    V, pm, g = _encoder_geometry(enc, img_feats, pts_feats, img_metas, pts_metas)
     # ---- forward with saved intermediates
     img = ops.conv3x3(img_feats.contiguous(), *pk['shared_conv_img'], cout=C, x_nhwc=False)
     pts = ops.conv3x3(pts_feats.contiguous(), *pk['shared_conv_pts'], cout=C, x_nhwc=False)
@@ -213,23 +244,17 @@ def _encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_
         saved.append(dict(img=img, pts=pts, i2p=i2p, p2p=p2p, warped=warped, p2i=p2i, i2i=i2i))
         img, pts = new_img, new_pts
     # ---- backward
-    one = torch.ones(1, device=dev)
-    add = lambda a, b: b if a is None else (a if b is None else ops.axpy(a.contiguous(), b.contiguous(), one))
-    zeros_i = lambda: torch.zeros(BV * h * w, C, device=dev)
-    zeros_p = lambda: torch.zeros(B * Y * X, C, device=dev)
-    gi = d_img.reshape(-1, C).contiguous() if d_img is not None else zeros_i()
-    gp = d_pts.reshape(-1, C).contiguous() if d_pts is not None else zeros_p()
+    gi, gp = _seed_rows(d_img, img), _seed_rows(d_pts, pts)
     layer_grads = []
     for lp, sv in zip(reversed(pk['layers']), reversed(saved)):
         img_r, pts_r = sv['img'].view(-1, C), sv['pts'].view(-1, C)
         lg = {}
         # fuse convolutions: new = Wf [a | b | c] + bf
-        wi, wp = lp['i_fuse'][0], lp['p_fuse'][0]
-        di3 = ops.linear([gi], _t_weight(wi, dev))                     # [M_i, 3C] = d p2i | d i2i | d img (direct)
-        dp3 = ops.linear([gp], _t_weight(wp, dev))                     # [M_p, 3C] = d i2p | d p2p | d pts (direct)
-        lg['i_fuse'] = (torch.cat([_wgrad(gi, sv['p2i']), _wgrad(gi, sv['i2i']), _wgrad(gi, img_r.contiguous())], 1), ops.col_sum(gi))
-        lg['p_fuse'] = (torch.cat([_wgrad(gp, sv['i2p'].view(-1, C)), _wgrad(gp, sv['p2p']), _wgrad(gp, pts_r.contiguous())], 1),
-                        ops.col_sum(gp))
+        bw = _fuse_bw_pack(lp)
+        di3 = ops.linear([gi], bw['i_fuse'])                           # [M_i, 3C] = d p2i | d i2i | d img (direct)
+        dp3 = ops.linear([gp], bw['p_fuse'])                           # [M_p, 3C] = d i2p | d p2p | d pts (direct)
+        lg['i_fuse'] = _layer_grads(gi, sv['p2i'], sv['i2i'], img_r)
+        lg['p_fuse'] = _layer_grads(gp, sv['i2p'].view(-1, C), sv['p2p'], pts_r)
         d_p2i, d_i2i, d_img_dir = (di3[:, k * C:(k + 1) * C].contiguous() for k in range(3))
         d_i2p, d_p2p, d_pts_dir = (dp3[:, k * C:(k + 1) * C].contiguous() for k in range(3))
         # image side
@@ -237,9 +262,9 @@ def _encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_
         r_pi = lcab_backward(lp['p2i'], img_r, sv['warped'].view(-1, C), BV, h, w, d_p2i)
         r_ip = i2p_backward(lp['i2p'], sv['pts'], sv['img'], pm, g.proj, V, g.in_hw, d_i2p.view(B, Y, X, C))
         r_pp = lcab_backward(lp['p_iml'], pts_r, pts_r, B, Y, X, d_p2p)
-        new_gi = add(add(add(d_img_dir, r_ii['d_target']), r_pi['d_target']), r_ip['d_img'].view(-1, C))
+        new_gi = _add(_add(_add(d_img_dir, r_ii['d_target']), r_pi['d_target']), r_ip['d_img'].view(-1, C))
         d_bev = ops.bev_sample_bwd(r_pi['d_source'].view(BV, h, w, C).contiguous(), g.grid, V, (B, Y, X, C))
-        new_gp = add(add(add(d_pts_dir, r_pp['d_target']), r_ip['d_pts'].view(-1, C)), d_bev.view(-1, C))
+        new_gp = _add(_add(_add(d_pts_dir, r_pp['d_target']), r_ip['d_pts'].view(-1, C)), d_bev.view(-1, C))
         lg.update(i_iml={k: v for k, v in r_ii.items() if not k.startswith('d_')},
                   p2i={k: v for k, v in r_pi.items() if not k.startswith('d_')},
                   p_iml={k: v for k, v in r_pp.items() if not k.startswith('d_')},
@@ -248,15 +273,10 @@ def _encoder_backward(enc, img_feats, pts_feats, img_metas, pts_metas, d_img, d_
         gi, gp = new_gi, new_gp
     layer_grads.reverse()
     if d_pts_conv is not None:
-        gp = add(gp, d_pts_conv.reshape(-1, C).contiguous())
-    # shared 3x3 convolutions: input gradients = convolution of the output gradient with the transposed, flipped kernels
-    wti = _conv3x3_transposed(pk['shared_conv_img'][0], Ci, dev)
-    wtp = _conv3x3_transposed(pk['shared_conv_pts'][0], Cp, dev)
-    d_img_feats = ops.conv3x3(gi.view(BV, h, w, C), wti, None, cout=Ci, x_nhwc=True)
-    d_pts_feats = ops.conv3x3(gp.view(B, Y, X, C), wtp, None, cout=Cp, x_nhwc=True)
-
-    shared = dict(img=conv3x3_wgrad(img_feats, gi, C), pts=conv3x3_wgrad(pts_feats, gp, C))
-    return dict(d_img_feats=d_img_feats, d_pts_feats=d_pts_feats, layers=layer_grads, shared_conv=shared)
+        gp = _add(gp, d_pts_conv.reshape(-1, C))
+    d_img_feats, g_img = _shared_conv_backward(gi, pk['shared_conv_img'][0], img_feats)
+    d_pts_feats, g_pts = _shared_conv_backward(gp, pk['shared_conv_pts'][0], pts_feats)
+    return dict(d_img_feats=d_img_feats, d_pts_feats=d_pts_feats, layers=layer_grads, shared_conv=dict(img=g_img, pts=g_pts))
 
 
 class LCABFunction(torch.autograd.Function):
@@ -277,29 +297,52 @@ class LCABFunction(torch.autograd.Function):
         return None, r['d_target'], r['d_source'], None, None, None
 
 
+# ---- decoder: the steps the query x BEV layer and the RCNN blocks share ------------------------------------------------------
+def _put(R, *named):
+    """Store (module name, (d weight, d bias)) pairs under the modules' state_dict keys."""
+    for module, (dW, db) in named:
+        R[module + '.weight'], R[module + '.bias'] = dW, db
+
+
+def _ffn_norm_backward(dy, z, gamma, f, act, x, w2t, w1t):
+    """Backward of y = LayerNorm(z), z = x + linear2(f), f = act(linear1(x)) from the saved z, f and x, the norm's weight and
+    the transposed weights; act = (ops.relu_bwd, saved output) or (ops.gelu_bwd, saved pre-activation).
+    -> (dx, (d gamma, d beta), linear2's (dW, db), linear1's (dW, db)); the residual joins dx in the GEMM epilogue."""
+    act_bwd, act_saved = act
+    dz, dgamma, dbeta = ops.ln_bwd(dy, z, gamma)
+    g2 = _layer_grads(dz, f)
+    dh = act_bwd(ops.linear([dz], w2t), act_saved)
+    g1 = _layer_grads(dh, x)
+    return ops.linear([dh], w1t, res=dz), (dgamma, dbeta), g2, g1
+
+
+def _self_attn_backward(dz, a, qkv, out_t, B, P, H):
+    """Backward of out_proj(a), a = unmasked attention over the P queries of each sample with the saved projections
+    qkv [B*P, 3C] -> (d qkv, out_proj's (dW, db)).  The in-projection stays with the caller: its sources differ."""
+    g_out = _layer_grads(dz, a)
+    C = qkv.shape[1] // 3
+    da = ops.linear([dz], out_t)
+    return ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da, B, P, H), g_out
+
+
 # ---- decoder: TransformerDecoderLayer (query x BEV) ---------------------------------------------------------------------
 def _dec_bw_pack(dec, pk):
     """Transposed weights of the layer's dX products and the constants of fold.decoder_layer_unfold, built once per pack."""
     if '_bw' in pk:
         return pk['_bw']
     layer = dec.decoder[0]
-    dev = pk['bce'].device
     C = dec.hidden_channel
-    T = lambda w: fold.Weight(fold._d(w).reshape(w.shape[0], -1).t().contiguous(), dev)
-    s = float(C // dec.num_heads) ** -0.5
-    w_in = fold._d(layer.self_attn.in_proj_weight).clone()
-    w_in[:C] *= s
-    w_x = fold._d(layer.multihead_attn.in_proj_weight).clone()
-    w_x[:C] *= s
-    Td = lambda w: fold.Weight(w.t().contiguous(), dev)
-    pk['_bw'] = dict(ffn2=T(layer.linear2.weight), ffn1=T(layer.linear1.weight), cross_out=T(layer.multihead_attn.out_proj.weight),
-                     self_out=T(layer.self_attn.out_proj.weight), cross_q=Td(w_x[:C]), kv=Td(w_x[C:]), self_in=Td(w_in),
-                     spe2=T(layer.self_posembed.position_embedding_head[3].weight),
-                     cpe2=T(layer.cross_posembed.position_embedding_head[3].weight),
-                     unfold=fold.decoder_layer_unfold_consts(layer, dec.num_heads, dev), one=torch.ones(1, device=dev))
+    T = _transposed
+    # the forward's weights as packed: q rows with head_dim^-0.5 folded in, and [W | W] over two sources where the same
+    # projection reads a row and its positional embedding
+    pk['_bw'] = dict(ffn1=T(pk['ffn'][0]), ffn2=T(pk['ffn'][2]), cross_out=T(pk['cross_out'][0]), self_out=T(pk['self_attn'][2]),
+                     cross_q=T(pk['cross_q'][0].w[:, :C]), kv=T(pk['cross_kv'][0]), self_in=T(pk['self_attn'][0].w[:, :C]),
+                     spe2=T(pk['self_pe'][2]), cpe2=T(layer.cross_posembed.position_embedding_head[3].weight.flatten(1)),
+                     unfold=fold.decoder_layer_unfold_consts(layer, dec.num_heads, pk['bce'].device))
     return pk['_bw']
 
 
+@_precise()
 def decoder_layer_backward(dec, query, query_pos, bev, grad_out):
     """Backward of the decoder's TransformerDecoderLayer (reference models/utils/decoder_utils.py:35-113, 116-495; the call
     self.decoder[0](query_feat, lidar_feat_flatten, query_pos, bev_pos) of deepinteraction_decoder.py), shared by the base
@@ -310,11 +353,6 @@ def decoder_layer_backward(dec, query, query_pos, bev, grad_out):
     dec.decoder[0], keyed and shaped as in its state_dict).  query_pos gets no gradient (a gather of the constant bev_pos).
     The layer is re-run eagerly with its intermediates kept; everything stays on the device, without host synchronisation
     after the first call of a pack."""
-    with _precise():
-        return _decoder_layer_backward(dec, query, query_pos, bev, grad_out)
-
-
-def _decoder_layer_backward(dec, query, query_pos, bev, grad_out):
     pk = dec.pack()
     C, H = dec.hidden_channel, dec.num_heads
     B, Y, X, _ = bev.shape
@@ -327,43 +365,38 @@ def _decoder_layer_backward(dec, query, query_pos, bev, grad_out):
     query, query_pos, bev = query.contiguous(), query_pos.contiguous(), bev.contiguous()
     sv = {}
     dec._layer(pk, query, query_pos, bev, B, P, saved=sv)
-    add = lambda a, b: ops.axpy(a.contiguous(), b.contiguous(), bw['one'])
     R, F = {}, {}
-    # norm3, FFN
-    dz3, R['norm3.weight'], R['norm3.bias'] = ops.ln_bwd(grad_out.contiguous(), sv['z3'], pk['norm3'][0])
-    R['linear2.weight'], R['linear2.bias'] = _wgrad(dz3, sv['f']), ops.col_sum(dz3)
-    df = ops.relu_bwd(ops.linear([dz3], bw['ffn2']), sv['f'])
-    R['linear1.weight'], R['linear1.bias'] = _wgrad(df, sv['q2']), ops.col_sum(df)
-    dq2 = ops.linear([df], bw['ffn1'], res=dz3)
+    # norm3, FFN (ReLU)
+    dq2, n3, l2, l1 = _ffn_norm_backward(grad_out.contiguous(), sv['z3'], pk['norm3'][0], sv['f'], (ops.relu_bwd, sv['f']),
+                                         sv['q2'], bw['ffn2'], bw['ffn1'])
+    _put(R, ('norm3', n3), ('linear2', l2), ('linear1', l1))
     # norm2, query x BEV cross attention
     dz2, R['norm2.weight'], R['norm2.bias'] = ops.ln_bwd(dq2, sv['z2'], pk['norm2'][0])
-    R['multihead_attn.out_proj.weight'], R['multihead_attn.out_proj.bias'] = _wgrad(dz2, sv['a2']), ops.col_sum(dz2)
+    _put(R, ('multihead_attn.out_proj', _layer_grads(dz2, sv['a2'])))
     da2 = ops.linear([dz2], bw['cross_out'])
     dqc, dkv = ops.xattn_bwd(sv['planes'], sv['a2'], sv['lse'], da2, B, P, HW, H)
-    F['cross_q'] = (_wgrad(dqc, torch.cat([sv['q1'], sv['qpe']], 1)), ops.col_sum(dqc))
-    F['cross_kv'] = (_wgrad(dkv, sv['kk']), ops.col_sum(dkv))
+    F['cross_q'] = _layer_grads(dqc, torch.cat([sv['q1'], sv['qpe']], 1))
+    F['cross_kv'] = _layer_grads(dkv, sv['kk'])
     tq = ops.linear([dqc], bw['cross_q'])               # the [Wq | Wq] pack: the same gradient for q1 and qpe
     d_bev = ops.linear([dkv], bw['kv'])                 # d kk [B*HW, C] = d bev
     # constant key positional embedding: d kpe = sum over the batch of d kk, back through its MLP over the grid positions
     dkpe = d_bev[:HW]
     for b in range(1, B):
-        dkpe = add(dkpe, d_bev[b * HW:(b + 1) * HW])
+        dkpe = _add(dkpe, d_bev[b * HW:(b + 1) * HW])
     cpe = pk['cross_pe']
     dh = ops.relu_bwd(ops.linear([dkpe.contiguous()], bw['cpe2']), cpe['hidden'])
-    F['cross_posembed'] = (_wgrad(dh, cpe['pos']), ops.col_sum(dh), _wgrad(dkpe.contiguous(), cpe['hidden']), ops.col_sum(dkpe))
+    F['cross_posembed'] = _layer_grads(dh, cpe['pos']) + _layer_grads(dkpe, cpe['hidden'])
     # norm1, self attention over the queries
-    dz1, R['norm1.weight'], R['norm1.bias'] = ops.ln_bwd(add(dz2, tq), sv['z1'], pk['norm1'][0])
-    R['self_attn.out_proj.weight'], R['self_attn.out_proj.bias'] = _wgrad(dz1, sv['a1']), ops.col_sum(dz1)
-    da1 = ops.linear([dz1], bw['self_out'])
-    qkv = sv['qkv']
-    dqkv = ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da1, B, P, H)
-    F['self_in'] = (_wgrad(dqkv, torch.cat([query, sv['qpe']], 1)), ops.col_sum(dqkv))
+    dz1, R['norm1.weight'], R['norm1.bias'] = ops.ln_bwd(_add(dz2, tq), sv['z1'], pk['norm1'][0])
+    dqkv, g_out = _self_attn_backward(dz1, sv['a1'], sv['qkv'], bw['self_out'], B, P, H)
+    _put(R, ('self_attn.out_proj', g_out))
+    F['self_in'] = _layer_grads(dqkv, torch.cat([query, sv['qpe']], 1))
     ts = ops.linear([dqkv], bw['self_in'])              # the [W | W] pack: the same gradient for query and qpe
-    d_query = add(dz1, ts)
-    dqpe = add(tq, ts)
+    d_query = _add(dz1, ts)
+    dqpe = _add(tq, ts)
     # self positional MLP
     dhs = ops.relu_bwd(ops.linear([dqpe], bw['spe2']), sv['hs'])
-    F['self_posembed'] = (_wgrad(dhs, query_pos), ops.col_sum(dhs), _wgrad(dqpe, sv['hs']), ops.col_sum(dqpe))
+    F['self_posembed'] = _layer_grads(dhs, query_pos) + _layer_grads(dqpe, sv['hs'])
     R.update(fold.decoder_layer_unfold(bw['unfold'], F))
     return dict(d_query=d_query, d_bev=d_bev.view(B, Y, X, C), grads=R)
 
@@ -389,24 +422,17 @@ class DecoderLayerFunction(torch.autograd.Function):
 
 
 # ---- decoder: PointRCNNBlock (the BEV refinement block of the MMPI layers) -----------------------------------------------
-def _rcnn_bw_pack(dec, bp, li):
+def _rcnn_bw_pack(dec, bp):
     """Transposed weights of the block's dX products, built once per pack.  The DynamicConv generator's transpose
     [C, 2*128*128] stays a plain tensor: its dX product (K = 32768 over B*P rows) runs as a split-K FFMA product."""
     if '_bw' in bp:
         return bp['_bw']
-    blk = dec.decode_head[li]
-    g = lambda n: getattr(blk, n + blk.sfx)
-    dev = bp['norm1'][0].device
     C = dec.hidden_channel
-    T = lambda w: fold.Weight(fold._d(w).t().contiguous(), dev)
-    s = float(C // dec.num_heads) ** -0.5
-    mha, dyn = g('dyconv_pre_self_attn'), g('dyconv')
-    w_in = fold._d(mha.in_proj_weight).clone()
-    w_in[:C] *= s                                   # the q rows _pack_mha folds the head_dim^-0.5 into
+    T = _transposed
+    s = float(C // dec.num_heads) ** -0.5           # folded into the q rows of the packed in-projection (_pack_mha)
     qscale = torch.cat([torch.full((C,), s, dtype=torch.float64), torch.ones(2 * C, dtype=torch.float64)])
-    bp['_bw'] = dict(ffn2=T(g('linear2').weight), ffn1=T(g('linear1').weight), dout=T(dyn.out_layer.weight),
-                     dyn=fold.dev(fold._d(dyn.dynamic_layer.weight).t(), dev), attn_out=T(mha.out_proj.weight),
-                     attn_in=fold.Weight(w_in.t().contiguous(), dev), qscale=fold.dev(qscale, dev))
+    bp['_bw'] = dict(ffn1=T(bp['ffn'][0]), ffn2=T(bp['ffn'][2]), dout=T(bp['dout'][0]), dyn=bp['dyn'][0].w.t().contiguous(),
+                     attn_in=T(bp['attn'][0]), attn_out=T(bp['attn'][2]), qscale=fold.dev(qscale, bp['norm1'][0].device))
     return bp['_bw']
 
 
@@ -434,6 +460,7 @@ def _bev_roi_params(dec):
     return dec._roi_params((0, 0))          # the image size enters the image-mode RoIs only
 
 
+@_precise()
 def point_rcnn_backward(dec, li, query, pred, bev, grad_out):
     """Backward of the base decoder's PointRCNNBlock (reference models/utils/decoder_utils.py:765-841; dec.decode_head[li],
     li = 1 or 3 in the base configuration), LayerNorms as they are, dropout off.
@@ -444,45 +471,37 @@ def point_rcnn_backward(dec, li, query, pred, bev, grad_out):
     from detached predictions), so pred gets no gradient.  The block is re-run eagerly with its intermediates kept;
     everything stays on the device, without host synchronisation after the first call of a pack."""
     bp, B, P = _point_rcnn_block(dec, li, query, bev)
-    with _precise():
-        return _point_rcnn_backward(dec, li, bp, query.contiguous(), pred.contiguous(), bev.contiguous(),
-                                    grad_out.contiguous(), B, P)
-
-
-def _point_rcnn_backward(dec, li, bp, query, pred, bev, grad_out, B, P):
+    query, pred, bev, grad_out = query.contiguous(), pred.contiguous(), bev.contiguous(), grad_out.contiguous()
     C, H = dec.hidden_channel, dec.num_heads
     _, Y, X, _ = bev.shape
     sv = {}
     dec._rcnn_block(bp, query, pred, bev, None, B, P, _bev_roi_params(dec), None, None, saved=sv)
-    bw = _rcnn_bw_pack(dec, bp, li)
+    bw = _rcnn_bw_pack(dec, bp)
     R = {}
     # norm3, FFN (GELU)
-    dz3, R['norm3_pts.weight'], R['norm3_pts.bias'] = ops.ln_bwd(grad_out, sv['z3'], bp['norm3'][0])
-    R['linear2_pts.weight'], R['linear2_pts.bias'] = _wgrad(dz3, sv['f']), ops.col_sum(dz3)
-    dh = ops.gelu_bwd(ops.linear([dz3], bw['ffn2']), sv['h'])
-    R['linear1_pts.weight'], R['linear1_pts.bias'] = _wgrad(dh, sv['q2']), ops.col_sum(dh)
-    dq2 = ops.linear([dh], bw['ffn1'], res=dz3)
+    dq2, n3, l2, l1 = _ffn_norm_backward(grad_out, sv['z3'], bp['norm3'][0], sv['f'], (ops.gelu_bwd, sv['h']), sv['q2'],
+                                         bw['ffn2'], bw['ffn1'])
+    _put(R, ('norm3_pts', n3), ('linear2_pts', l2), ('linear1_pts', l1))
     # norm2, DynamicConv: norm3 + ReLU, out_layer, the dynamic convolution, the parameter generator, RoIAlign
     dz2, R['norm2_pts.weight'], R['norm2_pts.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
     D = 'dyconv_pts.'
     dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
-    R[D + 'out_layer.weight'], R[D + 'out_layer.bias'] = _wgrad(dzd3, sv['flat']), ops.col_sum(dzd3)
+    _put(R, (D + 'out_layer', _layer_grads(dzd3, sv['flat'])))
     d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
     dn = ops.col_sum(d_norm).view(4, C)
     R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
-    R[D + 'dynamic_layer.weight'], R[D + 'dynamic_layer.bias'] = _wgrad(d_params, sv['q1']), ops.col_sum(d_params)
+    _put(R, (D + 'dynamic_layer', _layer_grads(d_params, sv['q1'])))
     dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
     d_bev = ops.roi_align_bwd(d_roi, sv['rois'], B, Y, X, 1.0)
     # norm1, self attention over the queries of a sample (BEV mode: one group, no masks)
     dz1, R['norm1_pts.weight'], R['norm1_pts.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
     A = 'dyconv_pre_self_attn_pts.'
-    R[A + 'out_proj.weight'], R[A + 'out_proj.bias'] = _wgrad(dz1, sv['a']), ops.col_sum(dz1)
-    qkv = sv['qkv']
-    dqkv = ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], ops.linear([dz1], bw['attn_out']), B, P, H)
+    dqkv, g_out = _self_attn_backward(dz1, sv['a'], sv['qkv'], bw['attn_out'], B, P, H)
+    _put(R, (A + 'out_proj', g_out))
     d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
     # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
-    R[A + 'in_proj_weight'] = _wgrad(dqkv, query) * bw['qscale'][:, None]
-    R[A + 'in_proj_bias'] = ops.col_sum(dqkv) * bw['qscale']
+    dW_in, db_in = _layer_grads(dqkv, query)
+    R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = dW_in * bw['qscale'][:, None], db_in * bw['qscale']
     return dict(d_query=d_query, d_bev=d_bev, grads=R)
 
 

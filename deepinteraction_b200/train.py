@@ -57,7 +57,7 @@ class ConvBNTrain:
         grads[id(conv.weight)] = dw.view_as(conv.weight)
         if bn.weight is not None:
             grads[id(bn.weight)], grads[id(bn.bias)] = dg, db
-        return ops.linear([dy], fold.Weight(w.t().contiguous(), w.device, lazy=True))
+        return ops.linear([dy], bw._transposed(w))
 
 
 class LCABTrain:
@@ -82,19 +82,15 @@ class LCABTrain:
 
     def backward(self, dO, grads):
         """-> (d target, d source)"""
-        q, k, v, A, (N, H, W) = self.saved
+        q, k, v, A, dims = self.saved
         self.saved = None
         dO = dO.contiguous()
-        dA = ops.win_dot(dO, v, N, H, W, self.ks)
-        dv = ops.win_scatter(A, dO, N, H, W, self.ks)
-        dS = ops.win_softmax_bwd(A, dA, self.scale)
-        dq = ops.win_gather(dS, k, N, H, W, self.ks)
-        dk = ops.win_scatter(dS, q, N, H, W, self.ks)
+        dq, dk, dv = bw._window_backward(q, k, v, A, dO, dims, self.ks, self.scale)
         if DEBUG[0]:
             self.dbg.update(dq=dq, dk=dk, dv=dv, dO=dO)
         d_t = self.q1.backward(self.q2.backward(dq, grads), grads)
         d_s = self.k1.backward(self.k2.backward(dk, grads), grads)
-        return d_t, _add(d_s, self.v.backward(dv, grads))
+        return d_t, bw._add(d_s, self.v.backward(dv, grads))
 
 
 class FuseTrain:
@@ -131,12 +127,6 @@ class GradSink(dict):
         self.on_grad(self.names[key], grad)
 
 
-def _add(a, b):
-    if a is None or b is None:
-        return b if a is None else a
-    return ops.axpy(a.contiguous(), b.contiguous(), torch.ones(1, device=a.device))
-
-
 def encoder_train_step(enc, img_feats, pts_feats, img_metas, pts_metas, grad_fn, debug=None, dropout_seed=None, on_grad=None):
     """One training-mode forward + backward of DeepInteractionEncoder (base model).
 
@@ -156,16 +146,10 @@ def encoder_train_step(enc, img_feats, pts_feats, img_metas, pts_metas, grad_fn,
 
 
 def _encoder_train_step(enc, img_feats, pts_feats, img_metas, pts_metas, grad_fn, debug=None, dropout_seed=None, on_grad=None):
-    from . import mmri
     dev = img_feats.device
     C = enc.hidden_channel
-    BV, Ci, h, w = img_feats.shape
-    B, Cp, Y, X = pts_feats.shape
-    V = BV // B
-    pm = enc._canon_pts_metas(pts_metas, dev)
-    pm['pts'] = [p.to(dev) for p in pts_metas['pts']]
-    g = mmri.Geometry(img_metas, pm, (h, w), (Y, X), dev)
-    g.wait()
+    (BV, _, h, w), (B, _, Y, X) = img_feats.shape, pts_feats.shape
+    V, pm, g = bw._encoder_geometry(enc, img_feats, pts_feats, img_metas, pts_metas)
     Wt = lambda t: fold.Weight(t, dev, lazy=True)
     d = lambda t: fold.dev(t, dev)
     conv_pack = lambda conv: (Wt(fold.pack_conv3x3(conv.weight.detach())), d(conv.bias.detach()))
@@ -205,18 +189,17 @@ def _encoder_train_step(enc, img_feats, pts_feats, img_metas, pts_metas, grad_fn
     # ---- backward
     names = {id(p): n for n, p in enc.named_parameters()}
     grads = {} if on_grad is None else GradSink(names, on_grad)
-    gi = d_img.reshape(-1, C).contiguous() if d_img is not None else torch.zeros(BV * h * w, C, device=dev)
-    gp = d_pts.reshape(-1, C).contiguous() if d_pts is not None else torch.zeros(B * Y * X, C, device=dev)
+    gi, gp = bw._seed_rows(d_img, img), bw._seed_rows(d_pts, pts)
     for L in reversed(layers):
         d_p2i, d_i2i, d_img_dir = L['i_fuse'].backward(gi, grads)
         d_i2p, d_p2p, d_pts_dir = L['p_fuse'].backward(gp, grads)
         t_ii, s_ii = L['i_iml'].backward(d_i2i, grads)
         t_pi, s_pi = L['p2i'].backward(d_p2i, grads)
-        r_ip = bw._i2p_backward(L['i2p'], L['pts'], L['img'], pm, g.proj, V, g.in_hw, d_i2p.view(B, Y, X, C), L['drop'])
+        r_ip = bw.i2p_backward(L['i2p'], L['pts'], L['img'], pm, g.proj, V, g.in_hw, d_i2p.view(B, Y, X, C), L['drop'])
         t_pp, s_pp = L['p_iml'].backward(d_p2p, grads)
-        gi = _add(_add(_add(_add(d_img_dir, t_ii), s_ii), t_pi), r_ip['d_img'].view(-1, C))
+        gi = bw._add(bw._add(bw._add(bw._add(d_img_dir, t_ii), s_ii), t_pi), r_ip['d_img'].view(-1, C))
         d_bev = ops.bev_sample_bwd(s_pi.view(BV, h, w, C).contiguous(), g.grid, V, (B, Y, X, C))
-        gp = _add(_add(_add(_add(d_pts_dir, t_pp), s_pp), r_ip['d_pts'].view(-1, C)), d_bev.view(-1, C))
+        gp = bw._add(bw._add(bw._add(bw._add(d_pts_dir, t_pp), s_pp), r_ip['d_pts'].view(-1, C)), d_bev.view(-1, C))
         if debug is not None:
             debug.setdefault('bwd', []).insert(0, dict(p2i=d_p2i, i2i=d_i2i, i2p=d_i2p, p2p=d_p2p, warped=s_pi))
         mha = L['mha']
@@ -229,12 +212,10 @@ def _encoder_train_step(enc, img_feats, pts_feats, img_metas, pts_metas, grad_fn
         grads[id(mha.in_proj_bias)] = f32(torch.cat([u['bq'], u['bk'], u['bv']], 0))
         grads[id(mha.out_proj.weight)], grads[id(mha.out_proj.bias)] = f32(u['Wo']), f32(u['bo'])
     if d_pts_conv is not None:
-        gp = _add(gp, d_pts_conv.reshape(-1, C).contiguous())
-    wti = bw._conv3x3_transposed(pk_img[0], Ci, dev)
-    wtp = bw._conv3x3_transposed(pk_pts[0], Cp, dev)
-    d_img_feats = ops.conv3x3(gi.view(BV, h, w, C), wti, None, cout=Ci, x_nhwc=True)
-    d_pts_feats = ops.conv3x3(gp.view(B, Y, X, C), wtp, None, cout=Cp, x_nhwc=True)
-    for conv, x, gr in ((enc.shared_conv_img, img_feats, gi), (enc.shared_conv_pts, pts_feats, gp)):
-        grads[id(conv.weight)], grads[id(conv.bias)] = bw.conv3x3_wgrad(x, gr, C)
+        gp = bw._add(gp, d_pts_conv.reshape(-1, C))
+    d_img_feats, g_img = bw._shared_conv_backward(gi, pk_img[0], img_feats)
+    d_pts_feats, g_pts = bw._shared_conv_backward(gp, pk_pts[0], pts_feats)
+    for conv, g_conv in ((enc.shared_conv_img, g_img), (enc.shared_conv_pts, g_pts)):
+        grads[id(conv.weight)], grads[id(conv.bias)] = g_conv
     return dict(outputs=outputs, d_img_feats=d_img_feats, d_pts_feats=d_pts_feats,
                 grads={names[k]: v for k, v in grads.items()})
