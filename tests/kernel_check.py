@@ -12,10 +12,39 @@ def _ops():
 
 
 def _capi(name, *args):
-    """Call a C entry point directly (the wrappers allocate their outputs; these tests pre-fill them)."""
+    """Call a C entry point directly (the wrappers allocate their outputs; these tests pre-fill them); returns its
+    status (a count where the entry point returns one)."""
     ops = _ops()
-    ops._call(name, *args, ops._stream())
+    rc = ops._call(name, *args, ops._stream())
     torch.cuda.synchronize()
+    return rc
+
+
+def _status(name, *args):
+    """The raw status of a C entry point, without raising on an error code (tests of the documented rejections)."""
+    from deepinteraction_b200 import _lib
+    ops = _ops()
+    rc = getattr(_lib.lib(), name)(*args, ops._stream())
+    torch.cuda.synchronize()
+    return rc
+
+
+class record_calls:
+    """`with record_calls() as calls:` lists (entry point, args) of every C call the ops wrappers issue inside."""
+
+    def __enter__(self):
+        ops = _ops()
+        self.calls, self.saved = [], ops._call
+
+        def rec(name, *args, **kw):
+            self.calls.append((name, args))
+            return self.saved(name, *args, **kw)
+        ops._call = rec
+        return self.calls
+
+    def __exit__(self, *a):
+        _ops()._call = self.saved
+        return False
 
 
 def row_err(got, want, scale, width=None):

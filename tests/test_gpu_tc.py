@@ -6,6 +6,7 @@ import torch
 import torch.nn.functional as F
 
 from conftest import rel_err
+from kernel_check import record_calls
 
 pytestmark = pytest.mark.gpu
 TIGHT = 5e-5
@@ -92,13 +93,18 @@ def test_conv3x3_tc_matches_float64(N, Cin, H, W, Cout, nhwc_in, act, tc_mode):
         ref = F.relu(ref)
     xin = x.permute(0, 2, 3, 1).contiguous() if nhwc_in else x
     Wt = fold.Weight(fold.pack_conv3x3(w), dev())
-    for direct in ((False,) if nhwc_in else (False, True)):     # NCHW inputs: via transposition, and read in place
+    # NCHW inputs: via transposition, and read in place where the direct kernel applies (W % 4 == 0)
+    for direct in ((False,) if nhwc_in or W % 4 else (False, True)):
         old = ops.NCHW_DIRECT[0]
         ops.NCHW_DIRECT[0] = direct
         try:
-            y = ops.conv3x3(xin.to(dev()), Wt, b.to(dev()), Cout, nhwc_in, False, act).cpu().permute(0, 3, 1, 2)
+            with record_calls() as calls:
+                y = ops.conv3x3(xin.to(dev()), Wt, b.to(dev()), Cout, nhwc_in, False, act).cpu().permute(0, 3, 1, 2)
         finally:
             ops.NCHW_DIRECT[0] = old
+        bf = ops.TC_BF16[0] and Cin % 64 == 0
+        assert [c[0] for c in calls if 'conv3x3' in c[0]] == ['di_conv3x3_tc%s%s_f32' % ('b' if bf else '',
+                                                                                        '_nchw' if direct else '')]
         e = rel_err(y, ref.float())
         print(f'conv_tc N={N} Cin={Cin} {H}x{W} direct={direct}: rel err {e:.2e}')
         assert e < TIGHT
