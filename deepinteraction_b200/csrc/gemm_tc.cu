@@ -7,13 +7,12 @@
 // mantissa bits kept, error ~1e-5) -- see the BF template flag below.  A plain TF32/BF16 product is not admissible:
 // the parity bar of this path is 1e-3 end to end over ~40 chained layers and includes exact top-k indices.
 // Same layers as gemm.cu: every 1x1 Conv(+BN)(+ReLU) / cat+conv pair (reference models/utils/encoder_utils.py:11-34,
-// models/necks/deepinteraction_encoder.py:26-32) and the 3x3 convs as implicit GEMM over pixel-major (NHWC) maps
-// (models/necks/deepinteraction_encoder.py:47-62, models/dense_heads/deepinteraction_decoder.py:83-101).
+// models/necks/deepinteraction_encoder.py:26-32) and the 3x3 convs over channel-major (NCHW) inputs as implicit GEMM
+// (variant ANCHW below); the 3x3 convs over pixel-major (NHWC) maps have their own kernel in conv_tc.cu.
 //
 // Persistent CTAs (at most one per SM) walk the 128 x 128 output tiles with a static stride; 384 threads in three
 // warpgroups, all hand-offs through mbarriers:
-//   warpgroup 0   TMA producer (one thread): per K chunk, box loads of fp32 A (2-D [rows,K] map, or a 4-D NHWC map
-//                 whose 8x16-pixel box shifted by the filter tap gives the zero padding for free) and of W_hi / W_lo
+//   warpgroup 0   TMA producer (one thread): per K chunk, box loads of fp32 A (2-D [rows,K] map) and of W_hi / W_lo
 //                 into a ring of 128B-swizzled K-major tiles (cp.async.bulk.tensor + mbarrier tx-count); L2 prefetch of
 //                 the next tile's A rows.  For K <= 128 the weight slice is loaded once and stays resident.
 //   warpgroups 1-2  consumers, 64 output rows each: landed A chunk -> registers (the wgmma A fragment, read through
@@ -46,7 +45,7 @@ struct TcParams {
   int nsrc;                 // linear: number of A sources (1..3)
   int k0, k1, k2;           // linear: K_s / KE per source; conv: k0 = Cin / KE.  (Scalars, not an array: a dynamically
                             // indexed kernel parameter makes ptxas copy the whole struct to LOCAL memory.)
-  int conv;                 // 1: 3x3 conv over an NHWC map (A map is 4-D)
+  int conv;                 // 1: 3x3 conv over an NCHW map (variant ANCHW, A map is 4-D)
   int H, W, tiles_x, tiles_y;  // conv geometry: tile = 8 rows x 16 cols of pixels
   int m_tiles, n_tiles;     // tile grid (m_tiles = images * tiles_y * tiles_x for conv)
   float* C;
@@ -195,27 +194,21 @@ gemm_tc_kernel_v3(const __grid_constant__ CUtensorMap mapA0, const __grid_consta
             DBG_STAMP(0, it);
             const uint32_t st = base + RING_OFF + s * STG;
             mbar_expect_tx(full(s), STG);
-            if (p.conv) {
-              const int tap = kc_all / p.k0, kc = kc_all - tap * p.k0;
-              tma_load_4d(st, &mapA0, full(s), kc * KE, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
-              if (BF) tma_load_4d(st + A_BYTES, &mapA0, full(s), kc * KE + 32, x0 + tap % 3 - 1, y0 + tap / 3 - 1, img);
-            } else {
-              int src = 0, kc = kc_all;
-              while (kc >= tc_kch(p, src)) {
-                kc -= tc_kch(p, src);
-                ++src;
-              }
-              const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
-              tma_load_2d(st, mp, full(s), kc * KE, m0);
-              if (BF) tma_load_2d(st + A_BYTES, mp, full(s), kc * KE + 32, m0);
+            int src = 0, kc = kc_all;
+            while (kc >= tc_kch(p, src)) {
+              kc -= tc_kch(p, src);
+              ++src;
             }
+            const CUtensorMap* mp = src == 0 ? &mapA0 : (src == 1 ? &mapA1 : &mapA2);
+            tma_load_2d(st, mp, full(s), kc * KE, m0);
+            if (BF) tma_load_2d(st + A_BYTES, mp, full(s), kc * KE + 32, m0);
             if (!WRES) {
               tma_load_2d(st + AL, &mapWhi, full(s), kc_all * KE, n0);
               tma_load_2d(st + AL + A_BYTES, &mapWlo, full(s), kc_all * KE, n0);
             }
           }
           const int nxt = tile + (int)gridDim.x;       // L2 prefetch of the next tile's A rows
-          if (nxt < num_tiles && !p.conv) {
+          if (nxt < num_tiles) {
             const int mt = nxt / p.n_tiles;
             for (int src = 0; src < p.nsrc; ++src)
               for (int kc = 0; kc < tc_kch(p, src); ++kc) {
@@ -419,19 +412,6 @@ bool make_map_2d(CUtensorMap* m, const float* ptr, long long rows, long long col
              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
 }
-// 4-D fp32 map over an NHWC tensor; box = 32 channels x 16 x-pixels x 8 y-pixels x 1 image
-bool make_map_nhwc(CUtensorMap* m, const float* ptr, int N, int H, int W, int C) {
-  EncodeTiledFn enc = get_encode();
-  if (!enc) return false;
-  cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)N};
-  cuuint64_t strides[3] = {(cuuint64_t)C * 4, (cuuint64_t)W * C * 4, (cuuint64_t)H * W * C * 4};
-  cuuint32_t box[4] = {TK, 16, 8, 1};
-  cuuint32_t estr[4] = {1, 1, 1, 1};
-  return enc(m, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 4, const_cast<float*>(ptr), dims, strides, box, estr,
-             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) == CUDA_SUCCESS;
-}
-
 // 2-D bf16 map over a row-major [rows, cols] weight (cols contiguous); box = 64 cols (128 B) x 128 rows
 bool make_map_2d_bf16(CUtensorMap* m, const void* ptr, long long rows, long long cols) {
   EncodeTiledFn enc = get_encode();
@@ -606,9 +586,10 @@ int conv3x3_tc_impl(const char* name, int bf, int x_nchw, const float* x, const 
     di_set_error("%s: shape/alignment not supported by the tensor-core path", name);
     return DI_ERR_UNSUPPORTED;
   }
+  if (!x_nchw) return conv3x3_nhwc(name, bf, x, w_hi, w_lo, bias, y, N, Cin, H, W, Cout, act, stream);
   CUtensorMap maps[5];
   long long K = 9ll * Cin;
-  bool made = (x_nchw ? make_map_nchw(&maps[0], x, N, H, W, Cin, KE) : make_map_nhwc(&maps[0], x, N, H, W, Cin));
+  bool made = make_map_nchw(&maps[0], x, N, H, W, Cin, KE);
   if (made) {
     if (bf) made = make_map_2d_bf16(&maps[3], w_hi, Cout, K) && make_map_2d_bf16(&maps[4], w_lo, Cout, K);
     else made = make_map_2d(&maps[3], (const float*)w_hi, Cout, K, K) && make_map_2d(&maps[4], (const float*)w_lo, Cout, K, K);

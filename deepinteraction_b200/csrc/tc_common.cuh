@@ -1,4 +1,4 @@
-// Hopper (sm_90a) tensor-core primitives shared by the dense kernels (gemm_tc.cu): mbarrier, TMA (cp.async.bulk.tensor)
+// Hopper (sm_90a) tensor-core primitives shared by the dense kernels (gemm_tc.cu, conv_tc.cu): mbarrier, TMA (cp.async.bulk.tensor)
 // and warpgroup MMA (wgmma) with the A operand in registers and B as a 128B-swizzled K-major shared-memory tile.
 #pragma once
 #include "common.cuh"
@@ -82,11 +82,19 @@ __device__ __forceinline__ uint64_t wgmma_desc(uint32_t smem_addr) {
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// all but the most recently committed group have completed
+__device__ __forceinline__ void wgmma_wait_one() { asm volatile("wgmma.wait_group.sync.aligned 1;" ::: "memory"); }
 // keeps the compiler from moving accumulator registers across the asynchronous wgmma window
 template <int N>
 __device__ __forceinline__ void fence_regs(float (&r)[N]) {
 #pragma unroll
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
+}
+// the same for register A fragments: keeps them (and their registers) live until this point
+template <int N>
+__device__ __forceinline__ void fence_regs(uint32_t (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+r"(r[i])::"memory");
 }
 
 // D[64 x 128] (+)= A[64 x k] * B[128 x k]^T for one warpgroup.  A: registers, the mma.m16n8k16 (bf16) / m16n8k8 (tf32)
@@ -113,6 +121,25 @@ __device__ __forceinline__ void wgmma_tf32_rs(float (&d)[64], const uint32_t (&a
       : "memory");
 }
 
+// The same products on a 16-column B tile (D[64 x 16], 8 accumulators per thread), for narrow outputs.
+__device__ __forceinline__ void wgmma_bf16_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1, 0;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
+      : "memory");
+}
+__device__ __forceinline__ void wgmma_tf32_rs(float (&d)[8], const uint32_t (&a)[4], uint64_t desc_b, uint32_t scale_d) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %13, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n16k8.f32.tf32.tf32 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7}, {%8, %9, %10, %11}, %12, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(scale_d)
+      : "memory");
+}
 
 // two fp32 -> packed bf16x2 (round to nearest even): low half = lo_elem, high half = hi_elem
 __device__ __forceinline__ uint32_t pack_bf16x2(float lo_elem, float hi_elem) {
@@ -141,5 +168,11 @@ inline EncodeTiledFn get_encode() {
 // CTAs a persistent tensor-core grid may use on the current device: its SM count, capped by di_tc_set_sm_limit
 // (gemm_tc.cu).  Returns DI_OK or an error status with the message set.
 int sm_budget(const char* name, int* sms);
+
+// 3x3 convolution over an NHWC map (conv_tc.cu), behind di_conv3x3_tc[b]_f32 once their arguments are checked:
+// x [N,H,W,Cin], w_hi / w_lo [Cout][9 * Cin] (bf = 1: bf16 hi / mid, Cin % 64 == 0; bf = 0: fp32 tf32 split,
+// Cin % 32 == 0), y [N,H,W,Cout], Cout % 4 == 0.
+int conv3x3_nhwc(const char* name, int bf, const float* x, const void* w_hi, const void* w_lo, const float* bias,
+                 float* y, int N, int Cin, int H, int W, int Cout, int act, cudaStream_t stream);
 
 }  // namespace tc

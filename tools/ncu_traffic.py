@@ -15,7 +15,8 @@ ENTRY = [('lcab_window_tc_kernel', 'di_lcab_window_tc_f32'), ('lcab_proj_kernel'
          ('lcab_window_pre_kernel', 'di_lcab_window_pre_f32'), ('msdeform_kernel', 'di_msdeform_f32'),
          ('i2p_attend_kernel', 'di_i2p_attend_f32'), ('bev_sample_kernel', 'di_bev_sample_f32'),
          ('cross_attn', 'di_cross_attn_f32'), ('dynconv_kernel', 'di_dynconv_f32'), ('seq_attn_kernel', 'di_seq_attn_f32'),
-         ('gemm_tc_kernel_v3', 'gemm_tc_kernel_v3 (di_linear_tc*/di_conv3x3_tc*)'), ('rows_mlp_kernel', 'di_rows_mlp_f32'),
+         ('gemm_tc_kernel_v3', 'gemm_tc_kernel_v3 (di_linear_tc*/di_conv3x3_tc*_nchw)'),
+         ('conv3x3_tc_kernel', 'conv3x3_tc_kernel (di_conv3x3_tc*_f32)'), ('rows_mlp_kernel', 'di_rows_mlp_f32'),
          ('depth_complete_kernel', 'di_depth_complete')]
 
 
