@@ -19,8 +19,12 @@ constexpr int BN_RL = 8;
 
 __device__ __forceinline__ float4 f4_add(float4 a, float4 b) { return make_float4(a.x + b.x, a.y + b.y, a.z + b.z, a.w + b.w); }
 
-// per row block and channel: n, mean, M2 (sum of squared deviations from the block mean).  One pass with the sums shifted by
-// the block's first row (a sample of the column, so |mean - pivot| ~ the spread and s2 - s1^2 / n does not cancel).
+// per row block and channel: pivot, mean - pivot and M2 (sum of squared deviations from the block mean); the final kernel
+// recomputes the block's row count from M.  Two passes over the block's rows: the first estimates the mean from the
+// deviations from the block's first row; that estimate becomes the pivot, and the second pass sums the deviations d from
+// it: M2 = sum d^2 - (sum d)^2 / n.  One pass shifted by the first row loses M2 to cancellation when that row is an
+// outlier.  The mean stays split because pivot + offset rounded to fp32 costs half an ulp of |mean|, which the merge turns
+// into spurious variance between blocks when |mean| >> spread.
 __global__ void __launch_bounds__(256)
 bn_stats_part_kernel(const float* __restrict__ y, long long M, int C, float* __restrict__ part) {
   __shared__ float4 sh1[BN_RL][32], sh2[BN_RL][32];
@@ -28,9 +32,23 @@ bn_stats_part_kernel(const float* __restrict__ y, long long M, int C, float* __r
   const int c = blockIdx.y * 128 + tx * 4;
   const long long rows = (M + gridDim.x - 1) / gridDim.x, m0 = blockIdx.x * rows, m1 = min(M, m0 + rows);
   const bool on = c < C && m0 < m1;
+  const float n = (float)max(0LL, m1 - m0), inv = n > 0.f ? 1.f / n : 0.f;
   float4 s1 = make_float4(0.f, 0.f, 0.f, 0.f), s2 = s1, p = s1;
   if (on) {
     p = ld4(y + m0 * C + c);
+#pragma unroll 4
+    for (long long m = m0 + ty; m < m1; m += BN_RL) {
+      const float4 v = ld4(y + m * C + c);
+      s1.x += v.x - p.x; s1.y += v.y - p.y; s1.z += v.z - p.z; s1.w += v.w - p.w;
+    }
+  }
+  sh1[ty][tx] = s1;
+  __syncthreads();
+  s1 = sh1[0][tx];
+  for (int r = 1; r < BN_RL; ++r) s1 = f4_add(s1, sh1[r][tx]);
+  p = make_float4(p.x + s1.x * inv, p.y + s1.y * inv, p.z + s1.z * inv, p.w + s1.w * inv);
+  s1 = make_float4(0.f, 0.f, 0.f, 0.f);
+  if (on) {
 #pragma unroll 4
     for (long long m = m0 + ty; m < m1; m += BN_RL) {
       const float4 v = ld4(y + m * C + c);
@@ -39,17 +57,17 @@ bn_stats_part_kernel(const float* __restrict__ y, long long M, int C, float* __r
       s2.x = fmaf(dx, dx, s2.x); s2.y = fmaf(dy, dy, s2.y); s2.z = fmaf(dz, dz, s2.z); s2.w = fmaf(dw, dw, s2.w);
     }
   }
+  __syncthreads();
   sh1[ty][tx] = s1;
   sh2[ty][tx] = s2;
   __syncthreads();
   if (ty != 0 || c >= C) return;
   for (int r = 1; r < BN_RL; ++r) { s1 = f4_add(s1, sh1[r][tx]); s2 = f4_add(s2, sh2[r][tx]); }
-  const float n = (float)max(0LL, m1 - m0), inv = n > 0.f ? 1.f / n : 0.f;
   const float a1[4] = {s1.x, s1.y, s1.z, s1.w}, a2[4] = {s2.x, s2.y, s2.z, s2.w}, pv[4] = {p.x, p.y, p.z, p.w};
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     float* o = part + ((size_t)blockIdx.x * C + c + k) * 3;
-    o[0] = n; o[1] = pv[k] + a1[k] * inv; o[2] = fmaxf(a2[k] - a1[k] * a1[k] * inv, 0.f);
+    o[0] = pv[k]; o[1] = a1[k] * inv; o[2] = fmaxf(a2[k] - a1[k] * a1[k] * inv, 0.f);
   }
 }
 
@@ -68,10 +86,11 @@ bn_stats_final_kernel(const float* __restrict__ part, int nblk, int C, long long
                       float* __restrict__ var, float* __restrict__ run_mean, float* __restrict__ run_var, float momentum) {
   const int c = blockIdx.x * 8 + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (c >= C) return;
+  const long long rows = (M + nblk - 1) / nblk;      // the row split of bn_stats_part_kernel
   double n = 0.0, mu = 0.0, m2 = 0.0;
   for (int b = lane; b < nblk; b += 32) {
     const float* p = part + ((size_t)b * C + c) * 3;
-    chan_merge(n, mu, m2, (double)p[0], (double)p[1], (double)p[2]);
+    chan_merge(n, mu, m2, (double)max(0LL, min(rows, M - b * rows)), (double)p[0] + (double)p[1], (double)p[2]);
   }
 #pragma unroll
   for (int o = 1; o < 32; o <<= 1) {

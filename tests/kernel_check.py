@@ -5,6 +5,8 @@ that row (>= max|b_row|).  A global max hides a wrong row whose values are small
 summed terms, not to their sum, which may cancel.  A row whose terms are all zero must be exactly zero."""
 import torch
 
+SENT = 0x7FA5A5A5                 # NaN bit pattern of the output canvases
+
 
 def _ops():
     from deepinteraction_b200 import ops
@@ -62,3 +64,17 @@ def row_err(got, want, scale, width=None):
 def same_bits(a, b):
     a, b = a.detach().cpu().contiguous(), b.detach().cpu().contiguous()
     return a.shape == b.shape and torch.equal(a.view(torch.int32), b.view(torch.int32))
+
+
+def canvas(rows, cols, pad_cols=8, pad_rows=3):
+    """(buffer, view): a [rows, cols] output view with ldc = cols + pad_cols inside a SENT-filled buffer."""
+    buf = torch.full((rows + pad_rows, cols + pad_cols), SENT, dtype=torch.int32, device='cuda').view(torch.float32)
+    return buf, buf[:rows, :cols]
+
+
+def outside_intact(buf, rows, cols):
+    """Every word of a canvas outside its [rows, cols] view still holds SENT."""
+    b = buf.view(torch.int32)
+    keep = torch.ones_like(b, dtype=torch.bool)
+    keep[:rows, :cols] = False
+    return bool((b[keep] == SENT).all())

@@ -27,11 +27,10 @@ import pytest
 import torch
 import torch.nn.functional as F
 
-from kernel_check import _capi, _status, record_calls, row_err, same_bits
+from kernel_check import SENT, _capi, _status, canvas, outside_intact, record_calls, row_err, same_bits
 
 pytestmark = pytest.mark.gpu
 
-SENT = 0x7FA5A5A5                 # NaN bit pattern of the output canvas
 DI_ERR_ARG, DI_ERR_UNSUPPORTED = -1, -3
 SM_LIMITS = (0, 1, 7, 131)        # 0 = one CTA per SM; 1 and 7 are below / not multiples of n_tiles = 3, 5
 
@@ -101,19 +100,6 @@ def tc_state(mode=3, sm_limit=0):
     finally:
         L.di_tc_set_mode(3)
         L.di_tc_set_sm_limit(int(os.environ.get('DI_B200_TC_SMS', '0')))
-
-
-def canvas(rows, cols, pad_cols=8, pad_rows=3):
-    """(buffer, view): a [rows, cols] output view with ldc = cols + pad_cols inside a sentinel-filled buffer."""
-    buf = torch.full((rows + pad_rows, cols + pad_cols), SENT, dtype=torch.int32, device=dev()).view(torch.float32)
-    return buf, buf[:rows, :cols]
-
-
-def outside_intact(buf, rows, cols):
-    b = buf.view(torch.int32)
-    keep = torch.ones_like(b, dtype=torch.bool)
-    keep[:rows, :cols] = False
-    return bool((b[keep] == SENT).all())
 
 
 def exact(got, want):

@@ -152,8 +152,9 @@ def test_lazy_weight_equals_eager_weight():
 
 
 def test_train_mode_batchnorm_formulas():
-    """The closed forms csrc/bn_train.cu implements (shifted one-pass block moments merged with Chan's formula; dy = gamma rstd
-    (g - mean(g) - xhat mean(g xhat))) against torch.nn.functional.batch_norm + autograd, in float64 on the host."""
+    """The closed forms csrc/bn_train.cu implements (block moments about the block's estimated mean, merged with Chan's
+    formula; dy = gamma rstd (g - mean(g) - xhat mean(g xhat))) against torch.nn.functional.batch_norm + autograd, in
+    float64 on the host."""
     import torch.nn.functional as F
     g_ = torch.Generator().manual_seed(4)
     M, C, eps = 203, 5, 1e-5
@@ -161,9 +162,11 @@ def test_train_mode_batchnorm_formulas():
     parts = []
     for m0 in range(0, M, 37):                                    # row blocks as the kernel forms them
         blk = y[m0:m0 + 37]
-        d = blk - blk[0]
-        s1, s2, n = d.sum(0), (d * d).sum(0), blk.shape[0]
-        parts.append((n, blk[0] + s1 / n, s2 - s1 * s1 / n))
+        n = blk.shape[0]
+        p = blk[0] + (blk - blk[0]).sum(0) / n                   # first pass: the pivot
+        d = blk - p
+        s1, s2 = d.sum(0), (d * d).sum(0)
+        parts.append((n, p + s1 / n, s2 - s1 * s1 / n))
     n, mu, m2 = 0, torch.zeros(C).double(), torch.zeros(C).double()
     for nb, mub, m2b in parts:
         d = mub - mu
