@@ -72,7 +72,7 @@ SIGNATURES = {
     'di_topk_f32': [_p, _p, _i, _i, _i, _p, _i, _p],
     'di_query_init_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_mha_small_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _p],
-    'di_mha_small_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _i, _i, _i, _i, _p],
+    'di_mha_small_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _p],
     'di_cross_attn_f32': [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_rows_finish_f32': [_p, _i, _ll, _i, _p, _p, _i, _p, _p, _p, _i, _p, _i, _i, _i, _f, _p],
     'di_rows_mlp_f32': [_p, _i, _i, _p, _i, _i, _p, _p, _i, _i, _p, _p, _i, _p, _i, _p, _p, _f, _i, _p, _p, _i, _i, _p],

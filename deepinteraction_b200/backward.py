@@ -15,7 +15,7 @@ import contextlib
 
 import torch
 
-from . import fold, ops
+from . import fold, geom, ops
 
 
 @contextlib.contextmanager
@@ -316,13 +316,14 @@ def _ffn_norm_backward(dy, z, gamma, f, act, x, w2t, w1t):
     return ops.linear([dh], w1t, res=dz), (dgamma, dbeta), g2, g1
 
 
-def _self_attn_backward(dz, a, qkv, out_t, B, P, H):
-    """Backward of out_proj(a), a = unmasked attention over the P queries of each sample with the saved projections
-    qkv [B*P, 3C] -> (d qkv, out_proj's (dW, db)).  The in-projection stays with the caller: its sources differ."""
+def _self_attn_backward(dz, a, qkv, out_t, B, P, H, onbits=None, win=None):
+    """Backward of out_proj(a), a = attention over the P queries of each sample (within the view groups of onbits / win
+    when given) with the saved projections qkv [B*P, 3C] -> (d qkv, out_proj's (dW, db)).  The in-projection stays with
+    the caller: its sources differ."""
     g_out = _layer_grads(dz, a)
     C = qkv.shape[1] // 3
     da = ops.linear([dz], out_t)
-    return ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da, B, P, H), g_out
+    return ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da, B, P, H, onbits, win), g_out
 
 
 # ---- decoder: TransformerDecoderLayer (query x BEV) ---------------------------------------------------------------------
@@ -421,7 +422,7 @@ class DecoderLayerFunction(torch.autograd.Function):
         return None, r['d_query'], None, r['d_bev']
 
 
-# ---- decoder: PointRCNNBlock (the BEV refinement block of the MMPI layers) -----------------------------------------------
+# ---- decoder: the V1 RCNN blocks, PointRCNNBlock (BEV) and ImageRCNNBlock (camera views) --------------------------------
 def _rcnn_bw_pack(dec, bp):
     """Transposed weights of the block's dX products, built once per pack.  The DynamicConv generator's transpose
     [C, 2*128*128] stays a plain tensor: its dX product (K = 32768 over B*P rows) runs as a split-K FFMA product."""
@@ -442,22 +443,81 @@ def _rcnn_bw_pack(dec, bp):
 _DYN_SPLITS = 64
 
 
-def _point_rcnn_block(dec, li, query, bev):
-    """-> (block pack, B, P); NotImplementedError before any launch for what point_rcnn_backward does not cover."""
+def _v1_rcnn_block(dec, li, query, maps, image):
+    """-> (block pack, B, P) of decode_head[li], a V1 ImageRCNNBlock (image) or PointRCNNBlock (not image) read from maps
+    ([B*V, h, w, C] image maps or the [B, Y, X, C] BEV map); NotImplementedError before any launch for what the backward
+    of that block does not cover."""
+    fn, kind = ('image_rcnn_backward', 'ImageRCNNBlock') if image else ('point_rcnn_backward', 'PointRCNNBlock')
     bp = dec.pack()['blocks'][li]
-    if bp['image'] or bp['v2']:
-        raise NotImplementedError('point_rcnn_backward covers the V1 PointRCNNBlock only (decode_head[%d] is %s)'
-                                  % (li, type(dec.decode_head[li]).__name__))
-    C, M, B = dec.hidden_channel, query.shape[0], bev.shape[0]
-    P = M // B
-    if C != 128 or bev.shape[3] != C or query.shape[1] != C or P > 512 or P * B != M:
-        raise NotImplementedError('point_rcnn_backward: C = 128 and P <= 512 queries per sample '
-                                  f'(got C={query.shape[1]}, rows={M}, B={B})')
+    if bp['image'] != image or bp['v2']:
+        raise NotImplementedError('%s covers the V1 %s only (decode_head[%d] is %s)'
+                                  % (fn, kind, li, type(dec.decode_head[li]).__name__))
+    C, M = dec.hidden_channel, query.shape[0]
+    B = maps.shape[0] // dec.num_views if image else maps.shape[0]
+    P = M // max(B, 1)
+    if (C != 128 or maps.shape[3] != C or query.shape[1] != C or P > 512 or P * B != M
+            or (image and B * dec.num_views != maps.shape[0])):
+        raise NotImplementedError(f'{fn}: the {kind} gradient takes C = 128 and P <= 512 queries per sample '
+                                  f'(got C={query.shape[1]}, rows={M}, maps={maps.shape[0]})')
     return bp, B, P
 
 
 def _bev_roi_params(dec):
     return dec._roi_params((0, 0))          # the image size enters the image-mode RoIs only
+
+
+def _rcnn_forward(dec, bp, query, pred, maps, img_metas, B, P, saved=None):
+    """dec._rcnn_block on the block's maps: the BEV map, or the image maps, whose RoIs also need the camera constants of
+    img_metas.  Those go to the device from pinned memory, without a host synchronisation (a pageable source would make
+    the copy synchronous)."""
+    if not bp['image']:
+        return dec._rcnn_block(bp, query, pred, maps, None, B, P, _bev_roi_params(dec), None, None, saved=saved)
+    proj, aux = (t.pin_memory().to(maps.device, non_blocking=True) for t in dec._camera_consts(img_metas))
+    prm = dec._roi_params(geom.input_hw(img_metas))
+    return dec._rcnn_block(bp, query, pred, None, maps, B, P, prm, proj, aux, saved=saved)
+
+
+def _v1_rcnn_backward(dec, bp, B, P, query, pred, maps, img_metas, grad_out):
+    """Backward of a V1 RCNN block (reference models/utils/decoder_utils.py:632-761 image, :765-841 BEV), LayerNorms as
+    they are, dropout off -> (d_query, d_maps, grads).  The block is re-run eagerly with its intermediates kept.  The two
+    kinds differ where _rcnn_block does: the maps the RoIs read and their scale, the view-group masks (image blocks:
+    attention within a view group, rows on no live view written as 0) and the parameter names."""
+    image = bp['image']
+    query, pred, maps, grad_out = (t.contiguous() for t in (query, pred, maps, grad_out))
+    C, H = dec.hidden_channel, dec.num_heads
+    sv = {}
+    _rcnn_forward(dec, bp, query, pred, maps, img_metas, B, P, saved=sv)
+    bw = _rcnn_bw_pack(dec, bp)
+    x = '' if image else '_pts'
+    masks = (sv['onbits'], sv['win']) if image else ()
+    if image:
+        grad_out = ops.rows_finish(grad_out, zero_if_neg=sv['win'])     # the forward writes those rows as 0 by selection
+    R = {}
+    # norm3, FFN (GELU)
+    dq2, n3, l2, l1 = _ffn_norm_backward(grad_out, sv['z3'], bp['norm3'][0], sv['f'], (ops.gelu_bwd, sv['h']), sv['q2'],
+                                         bw['ffn2'], bw['ffn1'])
+    _put(R, ('norm3' + x, n3), ('linear2' + x, l2), ('linear1' + x, l1))
+    # norm2, DynamicConv: norm3 + ReLU, out_layer, the dynamic convolution, the parameter generator, RoIAlign
+    dz2, R[f'norm2{x}.weight'], R[f'norm2{x}.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
+    D = f'dyconv{x}.'
+    dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
+    _put(R, (D + 'out_layer', _layer_grads(dzd3, sv['flat'])))
+    d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
+    dn = ops.col_sum(d_norm).view(4, C)
+    R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
+    _put(R, (D + 'dynamic_layer', _layer_grads(d_params, sv['q1'])))
+    dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
+    d_maps = ops.roi_align_bwd(d_roi, sv['rois'], *maps.shape[:3], 1.0 / dec.out_size_factor_img if image else 1.0)
+    # norm1, self attention over the queries of a sample (image blocks: within the view groups)
+    dz1, R[f'norm1{x}.weight'], R[f'norm1{x}.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
+    A = f'dyconv_pre_self_attn{x}.'
+    dqkv, g_out = _self_attn_backward(dz1, sv['a'], sv['qkv'], bw['attn_out'], B, P, H, *masks)
+    _put(R, (A + 'out_proj', g_out))
+    d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
+    # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
+    dW_in, db_in = _layer_grads(dqkv, query)
+    R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = dW_in * bw['qscale'][:, None], db_in * bw['qscale']
+    return d_query, d_maps, R
 
 
 @_precise()
@@ -470,39 +530,27 @@ def point_rcnn_backward(dec, li, query, pred, bev, grad_out):
     dec.decode_head[li], keyed and shaped as in its state_dict).  The RoIs are constants (the reference computes them
     from detached predictions), so pred gets no gradient.  The block is re-run eagerly with its intermediates kept;
     everything stays on the device, without host synchronisation after the first call of a pack."""
-    bp, B, P = _point_rcnn_block(dec, li, query, bev)
-    query, pred, bev, grad_out = query.contiguous(), pred.contiguous(), bev.contiguous(), grad_out.contiguous()
-    C, H = dec.hidden_channel, dec.num_heads
-    _, Y, X, _ = bev.shape
-    sv = {}
-    dec._rcnn_block(bp, query, pred, bev, None, B, P, _bev_roi_params(dec), None, None, saved=sv)
-    bw = _rcnn_bw_pack(dec, bp)
-    R = {}
-    # norm3, FFN (GELU)
-    dq2, n3, l2, l1 = _ffn_norm_backward(grad_out, sv['z3'], bp['norm3'][0], sv['f'], (ops.gelu_bwd, sv['h']), sv['q2'],
-                                         bw['ffn2'], bw['ffn1'])
-    _put(R, ('norm3_pts', n3), ('linear2_pts', l2), ('linear1_pts', l1))
-    # norm2, DynamicConv: norm3 + ReLU, out_layer, the dynamic convolution, the parameter generator, RoIAlign
-    dz2, R['norm2_pts.weight'], R['norm2_pts.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
-    D = 'dyconv_pts.'
-    dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
-    _put(R, (D + 'out_layer', _layer_grads(dzd3, sv['flat'])))
-    d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
-    dn = ops.col_sum(d_norm).view(4, C)
-    R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
-    _put(R, (D + 'dynamic_layer', _layer_grads(d_params, sv['q1'])))
-    dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
-    d_bev = ops.roi_align_bwd(d_roi, sv['rois'], B, Y, X, 1.0)
-    # norm1, self attention over the queries of a sample (BEV mode: one group, no masks)
-    dz1, R['norm1_pts.weight'], R['norm1_pts.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
-    A = 'dyconv_pre_self_attn_pts.'
-    dqkv, g_out = _self_attn_backward(dz1, sv['a'], sv['qkv'], bw['attn_out'], B, P, H)
-    _put(R, (A + 'out_proj', g_out))
-    d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
-    # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
-    dW_in, db_in = _layer_grads(dqkv, query)
-    R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = dW_in * bw['qscale'][:, None], db_in * bw['qscale']
+    bp, B, P = _v1_rcnn_block(dec, li, query, bev, False)
+    d_query, d_bev, R = _v1_rcnn_backward(dec, bp, B, P, query, pred, bev, None, grad_out)
     return dict(d_query=d_query, d_bev=d_bev, grads=R)
+
+
+@_precise()
+def image_rcnn_backward(dec, li, query, pred, img, img_metas, grad_out):
+    """Backward of the base decoder's ImageRCNNBlock (reference models/utils/decoder_utils.py:632-761; dec.decode_head[li],
+    li = 0 or 2 in the base configuration), LayerNorms as they are, dropout off.
+    dec: DeepInteractionDecoder on the GPU; query [B*P, C]: the rows the block reads; pred [B*P, NP]: the prediction rows its
+    RoIs come from (di_rcnn_rois_f32, image mode); img [B*V, h, w, C]: the image maps (pixel-major, as forward_rows takes
+    them); img_metas: the frame's camera metadata; grad_out [B*P, C].
+    -> dict(d_query [B*P, C], d_img [B*V, h, w, C] (through RoIAlign at 1 / out_size_factor_img), grads = {name: tensor}
+    for the 24 parameters of dec.decode_head[li], keyed and shaped as in its state_dict).  A query with win = w >= 0 (the
+    last live view it is on) attends over the queries of its sample on view w and reads its RoI from map b*V + w; a query
+    on no live view outputs the constant 0, so its grad_out row is ignored and its d_query row is 0.  The RoIs and view
+    groups are constants (the reference computes them from detached predictions), so pred gets no gradient.  Everything
+    stays on the device, without host synchronisation after the first call of a pack."""
+    bp, B, P = _v1_rcnn_block(dec, li, query, img, True)
+    d_query, d_img, R = _v1_rcnn_backward(dec, bp, B, P, query, pred, img, img_metas, grad_out)
+    return dict(d_query=d_query, d_img=d_img, grads=R)
 
 
 class PointRCNNFunction(torch.autograd.Function):
@@ -512,15 +560,34 @@ class PointRCNNFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, dec, li, query, pred, bev):
-        bp, B, P = _point_rcnn_block(dec, li, query, bev)
+        bp, B, P = _v1_rcnn_block(dec, li, query, bev, False)
         ctx.dec, ctx.li = dec, li
         ctx.save_for_backward(query, pred, bev)
         with _precise():
-            return dec._rcnn_block(bp, query.contiguous(), pred.contiguous(), bev.contiguous(), None, B, P,
-                                   _bev_roi_params(dec), None, None)[0]
+            return _rcnn_forward(dec, bp, query.contiguous(), pred.contiguous(), bev.contiguous(), None, B, P)[0]
 
     @staticmethod
     def backward(ctx, grad_out):
         query, pred, bev = ctx.saved_tensors
         r = point_rcnn_backward(ctx.dec, ctx.li, query, pred, bev, grad_out)
         return None, None, r['d_query'], None, r['d_bev']
+
+
+class ImageRCNNFunction(torch.autograd.Function):
+    """autograd wrapper: out [B*P, C] = dec.decode_head[li] (a V1 ImageRCNNBlock) with the forward schedule's kernels, bit
+    for bit; backward -> (d_query, d_img) through image_rcnn_backward, no gradient for pred or img_metas (the RoIs and view
+    groups are constants).  Parameter gradients are returned by image_rcnn_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, li, query, pred, img, img_metas):
+        bp, B, P = _v1_rcnn_block(dec, li, query, img, True)
+        ctx.dec, ctx.li, ctx.img_metas = dec, li, img_metas
+        ctx.save_for_backward(query, pred, img)
+        with _precise():
+            return _rcnn_forward(dec, bp, query.contiguous(), pred.contiguous(), img.contiguous(), img_metas, B, P)[0]
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        query, pred, img = ctx.saved_tensors
+        r = image_rcnn_backward(ctx.dec, ctx.li, query, pred, img, ctx.img_metas, grad_out)
+        return None, None, r['d_query'], None, r['d_img'], None

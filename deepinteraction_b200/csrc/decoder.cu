@@ -316,19 +316,28 @@ mha_small_kernel(const float* __restrict__ q, int ldq, const float* __restrict__
   }
 }
 
-// Backward of mha_small_kernel without group masks (the transformer layer's self-attention, decoder_utils.py:95-99).
-// Pass 1, one warp per (query i, head): recompute A_i = softmax(q_i K^T), dA_ij = dO_i . v_j, D_i = sum_j A_ij dA_ij,
-// dS_ij = A_ij (dA_ij - D_i), dq_i = sum_j dS_ij k_j; A and dS are stored key-major ([b, head, j, i]) for pass 2.
-// Pass 2, one warp per (key j, head): dk_j = sum_i dS_ij q_i, dv_j = sum_i A_ij dO_i.  Fixed summation orders (lanes
-// over a strided index range, then the warp butterfly): deterministic, no atomics.
+// Backward of mha_small_kernel (the self-attention of the transformer layer, decoder_utils.py:95-99, and of the RCNN
+// blocks, with the same optional group mask: key j is visible to query i iff win[i] >= 0 and (onbits[j] >> win[i]) & 1).
+// Pass 1, one warp per (query i, head): recompute A_i = softmax(q_i K^T) over the visible keys, dA_ij = dO_i . v_j,
+// D_i = sum_j A_ij dA_ij, dS_ij = A_ij (dA_ij - D_i), dq_i = sum_j dS_ij k_j; A and dS are stored key-major
+// ([b, head, j, i]) for pass 2, for the visible pairs only.  A query with win < 0 gets a zero dq row and writes nothing.
+// Pass 2, one warp per (key j, head): dk_j = sum_i dS_ij q_i, dv_j = sum_i A_ij dO_i over the queries that see key j,
+// tested here again (pass 1 leaves the invisible pairs of the workspace unwritten).  Neither pass reads the rows of a
+// masked pair.  Fixed summation orders (lanes over a strided index range, then the warp butterfly): deterministic, no
+// atomics; without a mask every pair is visible and the arithmetic is that of the unmasked form.
 template <int D>
 __global__ void __launch_bounds__(256)
 mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk, const float* __restrict__ v,
                        int ldv, const float* __restrict__ dout, int ldd, float* __restrict__ dq, int ldg, float* __restrict__ aw,
-                       float* __restrict__ sw, int B, int P, int Hh) {
+                       float* __restrict__ sw, const int* __restrict__ onbits, const int* __restrict__ win, int B, int P, int Hh) {
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (wid >= B * P * Hh) return;
   const int head = wid % Hh, bq = wid / Hh, b = bq / P, i = bq % P;
+  const int wq = win ? win[bq] : 0;
+  if (wq < 0) {
+    if (lane < D) dq[(size_t)bq * ldg + head * D + lane] = 0.f;
+    return;
+  }
   float qr[D], gr[D];
 #pragma unroll
   for (int d = 0; d < D; d += 4) {
@@ -338,13 +347,15 @@ mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __rest
   }
   constexpr int MAXK = 16;  // P <= 512
   float sc[MAXK], dav[MAXK];
+  unsigned vis = 0;         // bit n: key n * 32 + lane exists and is visible
   float m = -INFINITY;
 #pragma unroll
   for (int n = 0; n < MAXK; ++n) {
     const int j = n * 32 + lane;
     sc[n] = -INFINITY;
     dav[n] = 0.f;
-    if (j < P) {
+    if (j < P && (!onbits || ((onbits[b * P + j] >> wq) & 1))) {
+      vis |= 1u << n;
       const float* kr = k + (size_t)(b * P + j) * ldk + head * D;
       const float* vr = v + (size_t)(b * P + j) * ldv + head * D;
       float s = 0.f, da = 0.f;
@@ -363,10 +374,12 @@ mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __rest
   float l = 0.f;
 #pragma unroll
   for (int n = 0; n < MAXK; ++n) {
-    sc[n] = n * 32 + lane < P ? expf(sc[n] - m) : 0.f;
+    sc[n] = (vis >> n) & 1 ? expf(sc[n] - m) : 0.f;
     l += sc[n];
   }
-  const float inv = 1.f / warp_sum(l);
+  l = warp_sum(l);
+  // a group that hides every key: zero weights and gradients, as the forward writes a zero row
+  const float inv = onbits && !(l > 0.f) ? 0.f : 1.f / l;
   float dsum = 0.f;
 #pragma unroll
   for (int n = 0; n < MAXK; ++n) {
@@ -381,7 +394,7 @@ mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __rest
 #pragma unroll
   for (int n = 0; n < MAXK; ++n) {
     const int j = n * 32 + lane;
-    if (j < P) {
+    if ((vis >> n) & 1) {
       const float ds = sc[n] * (dav[n] - dsum);
       aw[col + (size_t)j * P] = sc[n];
       sw[col + (size_t)j * P] = ds;
@@ -404,16 +417,22 @@ template <int D>
 __global__ void __launch_bounds__(256)
 mha_small_bwd_kv_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ dout, int ldd,
                         const float* __restrict__ aw, const float* __restrict__ sw, float* __restrict__ dk,
-                        float* __restrict__ dv, int ldg, int B, int P, int Hh) {
+                        float* __restrict__ dv, int ldg, const int* __restrict__ onbits, const int* __restrict__ win,
+                        int B, int P, int Hh) {
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
   if (wid >= B * P * Hh) return;
   const int head = wid % Hh, bj = wid / Hh, b = bj / P, j = bj % P;
+  const int bits = onbits ? onbits[bj] : 0;
   const float* ar = aw + ((size_t)(b * Hh + head) * P + j) * P;
   const float* sr = sw + ((size_t)(b * Hh + head) * P + j) * P;
   float ak[D], av[D];
 #pragma unroll
   for (int d = 0; d < D; ++d) ak[d] = av[d] = 0.f;
   for (int i = lane; i < P; i += 32) {
+    if (onbits) {
+      const int wi = win[b * P + i];
+      if (wi < 0 || !((bits >> wi) & 1)) continue;
+    }
     const float a = ar[i], ds = sr[i];
     const float* qr = q + (size_t)(b * P + i) * ldq + head * D;
     const float* gr = dout + (size_t)(b * P + i) * ldd + head * D;
@@ -1755,20 +1774,23 @@ int di_mha_small_f32(const float* q, int ldq, const float* k, int ldk, const flo
   return DI_OK;
 }
 
-// Backward of di_mha_small_f32 without group masks: dout [B*P, ldd] -> dq / dk / dv rows [B*P, ldg] (e.g. the three
-// column blocks of one [B*P, 3C] gradient); work: float [2 * B * heads * P * P].
+// Backward of di_mha_small_f32 with the same optional group mask (onbits, win): dout [B*P, ldd] -> dq / dk / dv rows
+// [B*P, ldg] (e.g. the three column blocks of one [B*P, 3C] gradient); work: float [2 * B * heads * P * P].
 int di_mha_small_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout, int ldd,
-                         float* dq, float* dk, float* dv, int ldg, float* work, int B, int P, int heads, int head_dim,
-                         cudaStream_t stream) {
+                         float* dq, float* dk, float* dv, int ldg, float* work, const int* onbits, const int* win, int B, int P,
+                         int heads, int head_dim, cudaStream_t stream) {
   DI_CHECK_ARG(q && k && v && dout && dq && dk && dv && work && B > 0 && P > 0 && heads > 0 && head_dim == 16 && P <= 512,
                "di_mha_small_bwd_f32: unsupported shape (head_dim=%d P=%d)", head_dim, P);
   DI_CHECK_ARG(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldd % 4 == 0, "di_mha_small_bwd_f32: strides must be multiples of 4");
+  DI_CHECK_ARG((onbits == nullptr) == (win == nullptr), "di_mha_small_bwd_f32: onbits and win go together");
   const int warps = B * P * heads;
   float* aw = work;
   float* sw = work + (size_t)B * heads * P * P;
-  mha_small_bwd_q_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, ldg, aw, sw, B, P, heads);
+  mha_small_bwd_q_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, ldg, aw, sw, onbits,
+                                                                    win, B, P, heads);
   DI_CHECK_LAUNCH("di_mha_small_bwd_f32");
-  mha_small_bwd_kv_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, dout, ldd, aw, sw, dk, dv, ldg, B, P, heads);
+  mha_small_bwd_kv_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, dout, ldd, aw, sw, dk, dv, ldg, onbits, win, B, P,
+                                                                     heads);
   DI_CHECK_LAUNCH("di_mha_small_bwd_f32 (keys)");
   return DI_OK;
 }

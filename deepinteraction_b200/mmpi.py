@@ -535,8 +535,8 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         """One RCNN block of the MMPI layers (decoder_utils.py:632-1089) on query rows: prev [B*P, C], pred [B*P, NP] (the
         previous layer's predictions, which give the RoIs), new_pts [B, Y, X, C] (BEV blocks) or img [B*V, h, w, C] (image
         blocks) -> (rows [B*P, C], rois [B*P, 5], win [B*P]).  The one implementation of the block, for the forward
-        schedule and for the eager re-run of backward.point_rcnn_backward; saved (a dict, V1 blocks) additionally stores
-        the values the backward needs, with the returned rows unchanged."""
+        schedule and for the eager re-run of backward.point_rcnn_backward and backward.image_rcnn_backward; saved (a dict,
+        V1 blocks) additionally stores the values the backward needs, with the returned rows unchanged."""
         C, H, V = self.hidden_channel, self.num_heads, self.num_views
         if bp['image']:
             rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 0, prm, proj, aux)
@@ -574,7 +574,7 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
             # pre-norm sums and the FFN's hidden rows, which the fused row kernels do not return
             h = self._mlp([q2], f1w, f1b)
             f = self._mlp([q2], f1w, f1b, ops.ACT_GELU)
-            saved.update(rois=rois, qkv=qkv, a=a, z1=self._mlp([a], wo, bo, res=prev), q1=q1, params=params, roi=roi,
+            saved.update(rois=rois, win=win, onbits=onbits, qkv=qkv, a=a, z1=self._mlp([a], wo, bo, res=prev), q1=q1, params=params, roi=roi,
                          flat=flat, part=part, zd3=ops.rows_finish(part, bias=bp['dout'][1]), t=t,
                          z2=ops.rows_finish(t, res=q1), q2=q2, h=h, f=f, z3=self._mlp([f], f2w, f2b, res=q2))
         return q, rois, win

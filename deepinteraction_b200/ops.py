@@ -911,15 +911,15 @@ def xattn_bwd(planes, out, lse, dout, B, P, HW, heads, dkv=None):
     return dq, dkv
 
 
-def mha_small_bwd(q, k, v, dout, B, P, heads):
-    """Gradient of mha_small without group masks: -> dqkv [B*P, 3C] = dq | dk | dv."""
+def mha_small_bwd(q, k, v, dout, B, P, heads, onbits=None, win=None):
+    """Gradient of mha_small, with the same optional group mask (onbits, win): -> dqkv [B*P, 3C] = dq | dk | dv."""
     C = q.shape[1]
     dqkv = torch.empty(B * P, 3 * C, device=q.device, dtype=torch.float32)
     work = torch.empty(2 * B * heads * P * P, device=q.device, dtype=torch.float32)
     (pq, lq), (pk, lk), (pv, lv), (pd, ld) = _rows(q), _rows(k), _rows(v), _rows(dout)
     base = dqkv.data_ptr()
     _call('di_mha_small_bwd_f32', pq, lq, pk, lk, pv, lv, pd, ld, ctypes.c_void_p(base), ctypes.c_void_p(base + 4 * C),
-          ctypes.c_void_p(base + 8 * C), 3 * C, _ptr(work), B, P, heads, C // heads, _stream(), launches=2)
+          ctypes.c_void_p(base + 8 * C), 3 * C, _ptr(work), _ptr(onbits), _ptr(win), B, P, heads, C // heads, _stream(), launches=2)
     return dqkv
 
 

@@ -252,10 +252,12 @@ int di_query_init_f32(const float* feat, const int* top, const float* heat, cons
 /* self-attention among the queries of a sample (models/utils/decoder_utils.py:95-99, :745, :826) */
 int di_mha_small_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo,
                      const int* onbits, const int* win, int B, int P, int heads, int head_dim, cudaStream_t stream);
-/* its backward without group masks: dout -> dq, dk, dv rows [B*P, ldg]; work: float [2 * B * heads * P * P]; deterministic */
+/* its backward: dout -> dq, dk, dv rows [B*P, ldg]; work: float [2 * B * heads * P * P]; deterministic.  onbits / win: the
+ * forward's optional group mask (both or neither): key j is visible to query i iff win[i] >= 0 and bit win[i] of onbits[j]
+ * is set; a query with win < 0 gets dq = 0, a key no query sees dk = dv = 0, and the rows of masked pairs are not read. */
 int di_mha_small_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout, int ldd,
-                         float* dq, float* dk, float* dv, int ldg, float* work, int B, int P, int heads, int head_dim,
-                         cudaStream_t stream);
+                         float* dq, float* dk, float* dv, int ldg, float* work, const int* onbits, const int* win, int B, int P,
+                         int heads, int head_dim, cudaStream_t stream);
 /* query x BEV cross attention (models/utils/decoder_utils.py:101-103, 466-488) */
 int di_cross_attn_f32(const float* q, const float* kv, float* part, float* out, int B, int P, int HW, int C, int heads,
                       int nsplit, cudaStream_t stream);

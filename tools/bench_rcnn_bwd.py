@@ -1,17 +1,22 @@
-"""Time the backward of the decoder's PointRCNNBlock on one GPU, next to the floors of its two new kernels.
+"""Time the backward of the decoder's V1 RCNN blocks on one GPU, next to the floors of their kernels.
 
-    python tools/bench_rcnn_bwd.py [--batches 1 2] [--iters 20] [--warmup 5] [--floors-only]
+    python tools/bench_rcnn_bwd.py [--block point|image] [--batches 1 2] [--iters 20] [--warmup 5] [--floors-only]
 
-At the base shapes (P = 200 queries, 180 x 180 BEV, C = 128) and per batch size, CUDA events time
+At the base shapes (P = 200 queries, C = 128) and per batch size, CUDA events time, for --block point (the default;
+decode_head[1], a PointRCNNBlock on the 180 x 180 BEV map)
   * di_roi_align_bwd_f32 (the RoIAlign gradient into the BEV map),
   * di_dynconv_bwd_f32 (the DynamicConv gradient, forward recomputed per query),
   * the whole backward.point_rcnn_backward (eager re-run of the block + every gradient product),
-  * the forward block (mmpi.DeepInteractionDecoder._rcnn_block as the schedule runs it), for comparison.
-The two kernels are printed with two floors computed from the shapes: their bytes at the data-sheet HBM bandwidth of the
-H100 SXM (3.35 TB/s) and their fp32 FLOPs at the data-sheet dense FP32 rate (67 TFLOP/s); the larger floor bounds the
-kernel.  The RoI rows come from prediction rows with boxes of 0.4 - 4.5 m (doubled in BEV mode, as the block does) spread
-over the map.  The GPU name, power limit and maximum SM clock come from nvidia-smi in the same run.  There is no CPU path:
-without a GPU the script fails (after printing the floors with --floors-only).
+  * the forward block (mmpi.DeepInteractionDecoder._rcnn_block as the schedule runs it), for comparison;
+and for --block image (decode_head[0], an ImageRCNNBlock on 6 x 112 x 200 image maps of a 6-camera rig, 448 x 800 inputs)
+  * di_mha_small_bwd_f32 with the block's view-group masks,
+  * di_roi_align_bwd_f32 into the B * 6 image maps at scale 1/4,
+  * the whole backward.image_rcnn_backward and the forward block.
+The RoIAlign and DynamicConv gradients are printed with two floors computed from the shapes: their bytes at the data-sheet
+HBM bandwidth of the H100 SXM (3.35 TB/s) and their fp32 FLOPs at the data-sheet dense FP32 rate (67 TFLOP/s); the larger
+floor bounds the kernel.  The RoI rows come from prediction rows with boxes of 0.4 - 4.5 m (doubled in BEV mode, as the
+block does) spread over the map.  The GPU name, power limit and maximum SM clock come from nvidia-smi in the same run.
+There is no CPU path: without a GPU the script fails (after printing the floors with --floors-only).
 """
 import argparse
 import json
@@ -27,20 +32,74 @@ from tools.bench_decoder_layer_bwd import _decoder, _time, gpu_info   # noqa: E4
 HBM_BPS = 3.35e12          # H100 SXM data sheet
 FP32_FLOPS = 67e12         # H100 SXM data sheet, dense FP32 (FFMA)
 P, Y, X, C = 200, 180, 180, 128
-LI = 1                     # decode_head[1]: the first PointRCNNBlock
+V, IMG_IN, IMG_HW = 6, (448, 800), (112, 200)
+LI = {'point': 1, 'image': 0}      # decode_head[1]: the first PointRCNNBlock, decode_head[0]: the first ImageRCNNBlock
 
 
-def floors(B):
+def floors(B, block='point'):
     """-> dict of (bytes, flops, floor_bytes_us, floor_flops_us) per kernel, from the shapes only."""
     n = B * P
-    roi_bytes = 4 * (n * 49 * C + B * Y * X * C + n * 5)          # d_out read, d_maps written, RoI rows
+    map_px = B * (V * IMG_HW[0] * IMG_HW[1] if block == 'image' else Y * X)
+    roi_bytes = 4 * (n * 49 * C + map_px * C + n * 5)             # d_out read, d_maps written, RoI rows
     roi_flops = 2 * 4 * 4 * 49 * C * n                             # 4 samples x 4 taps per bin, one FMA per channel
     dyn_bytes = 4 * (3 * n * 49 * C + 2 * n * 2 * C * C + n * 4 * C)   # roi, d_out, d_roi; params, d_params; partials
     dyn_flops = 6 * 2 * n * 49 * C * C                             # 2 products recomputed, 4 gradient products
     out = {}
-    for name, nbytes, flops in (('roi_align_bwd', roi_bytes, roi_flops), ('dynconv_bwd', dyn_bytes, dyn_flops)):
+    kernels = [('roi_align_bwd', roi_bytes, roi_flops)] + ([('dynconv_bwd', dyn_bytes, dyn_flops)] if block == 'point' else [])
+    for name, nbytes, flops in kernels:
         out[name] = dict(bytes=nbytes, flops=flops, floor_bytes_us=nbytes / HBM_BPS * 1e6, floor_flops_us=flops / FP32_FLOPS * 1e6)
     return out
+
+
+def image_inputs(m, B, g, d):
+    """-> (image maps [B*V, 112, 200, C], the camera metadata of synth.camera_rig(6, (448, 800)), prediction rows whose
+    centres spread over the BEV map at heights of -1.5 - 0.5 m), drawn with the CPU generator g."""
+    import numpy as np
+    import torch
+    from deepinteraction_b200 import synth
+    n = B * P
+    rig = synth.camera_rig(V, IMG_IN)
+    metas = [dict(lidar2img=[r.astype(np.float32) for r in rig], input_shape=IMG_IN, img_shape=[(*IMG_IN, 3)] * V)
+             for _ in range(B)]
+    pred = torch.randn(n, m.NP, generator=g)
+    pred[:, 0] = torch.rand(n, generator=g) * X
+    pred[:, 1] = torch.rand(n, generator=g) * Y
+    pred[:, 2] = torch.rand(n, generator=g) * 2 - 1.5
+    pred[:, 3:6] = torch.rand(n, 3, generator=g) * 2.5 - 1.0
+    img = torch.randn(B * V, *IMG_HW, C, generator=g)
+    return img.to(d), metas, pred.to(d)
+
+
+def run_image(B, iters, warmup):
+    import torch
+    from deepinteraction_b200 import backward, ops
+    d = torch.device('cuda')
+    g = torch.Generator().manual_seed(B)
+    m = _decoder()
+    bp = m.pack()['blocks'][LI['image']]
+    n = B * P
+    img, metas, pred = image_inputs(m, B, g, d)
+    query, grad = (torch.randn(n, C, generator=g).to(d) for _ in range(2))
+    sv = {}
+    with backward._precise():
+        backward._rcnn_forward(m, bp, query, pred, img, metas, B, P, saved=sv)
+    qkv, da = sv['qkv'], torch.randn(n, C, generator=g).to(d)
+    d_roi = torch.randn(n, 49, C, generator=g).to(d)
+    res = {}
+    res['mha_small_bwd_masked'] = _time(lambda: ops.mha_small_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da, B, P,
+                                                                  m.num_heads, sv['onbits'], sv['win']), iters, warmup)
+    res['roi_align_bwd'] = _time(lambda: ops.roi_align_bwd(d_roi, sv['rois'], B * V, *IMG_HW, 1.0 / m.out_size_factor_img),
+                                 iters, warmup)
+    res['image_rcnn_backward'] = _time(lambda: backward.image_rcnn_backward(m, LI['image'], query, pred, img, metas, grad),
+                                       iters, warmup)
+
+    def fwd():
+        with backward._precise():                    # the schedule's precision: 3xTF32 products
+            backward._rcnn_forward(m, bp, query, pred, img, metas, B, P)
+    res['forward_block'] = _time(fwd, iters, warmup)
+    live = sv['win'] >= 0
+    print('B=%d view groups: %d of %d queries on a live view' % (B, int(live.sum()), n))
+    return res
 
 
 def run(B, iters, warmup):
@@ -49,7 +108,8 @@ def run(B, iters, warmup):
     d = torch.device('cuda')
     g = torch.Generator(device=d).manual_seed(B)
     m = _decoder()
-    bp = m.pack()['blocks'][LI]
+    li = LI['point']
+    bp = m.pack()['blocks'][li]
     n = B * P
     pred = torch.randn(n, m.NP, device=d, generator=g)
     pred[:, 0] = torch.rand(n, device=d, generator=g) * X
@@ -67,7 +127,7 @@ def run(B, iters, warmup):
     res = {}
     res['roi_align_bwd'] = _time(lambda: ops.roi_align_bwd(d_roi, rois, B, Y, X, 1.0), iters, warmup)
     res['dynconv_bwd'] = _time(lambda: ops.dynconv_bwd(roi, params, *bp['dn1'], *bp['dn2'], d_flat), iters, warmup)
-    res['point_rcnn_backward'] = _time(lambda: backward.point_rcnn_backward(m, LI, query, pred, bev, grad), iters, warmup)
+    res['point_rcnn_backward'] = _time(lambda: backward.point_rcnn_backward(m, li, query, pred, bev, grad), iters, warmup)
 
     def fwd():
         with backward._precise():                    # the schedule's precision: 3xTF32 products
@@ -78,12 +138,13 @@ def run(B, iters, warmup):
 
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
+    ap.add_argument('--block', choices=['point', 'image'], default='point')
     ap.add_argument('--batches', type=int, nargs='+', default=[1, 2])
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--floors-only', action='store_true', help='print the floors and stop before touching the GPU')
     a = ap.parse_args(argv)
-    fl = {B: floors(B) for B in a.batches}
+    fl = {B: floors(B, a.block) for B in a.batches}
     for B in a.batches:
         for name, f in fl[B].items():
             print('B=%d %-14s floors: bytes %.1f MB -> %.1f us, fp32 %.2f GFLOP -> %.1f us (bound: %s)' % (
@@ -96,7 +157,7 @@ def main(argv=None):
         raise RuntimeError('bench_rcnn_bwd: no CUDA device (the kernels have no CPU path)')
     print('GPU (name, power limit, max SM clock):', gpu_info())
     for B in a.batches:
-        res = run(B, a.iters, a.warmup)
+        res = (run_image if a.block == 'image' else run)(B, a.iters, a.warmup)
         for name, (med, best) in res.items():
             f = fl[B].get(name)
             extra = ''
