@@ -123,8 +123,11 @@ __global__ void match_cost_kernel(const float* __restrict__ boxes, int nb, const
 // ---------------------------------------------------------------------------------------------------------------------
 // Rectangular linear sum assignment (shortest augmenting paths with dual variables; the formulation of D. F. Crouse,
 // "On implementing 2D rectangular assignment algorithms", 2016, which scipy.optimize.linear_sum_assignment implements).
-// One warp per (sample, layer) problem, float64 like scipy.  The problem is oriented so that the outer loop runs over
-// the smaller side (the ground-truth boxes, usually).  gt_inds [B, LP]: 0 = background, j + 1 = matched to box j.
+// One warp per (sample, layer) problem, float64 like scipy.  Ties are broken as scipy breaks them, because the reference's
+// matching is scipy's: the [P, G] cost matrix is transposed only when G < P (so the outer loop runs over the smaller
+// side), and each step scans the unvisited columns in scipy's `remaining` order (reversed at the start of each row,
+// shrunk by swap-removal), taking the first column of least cost unless a later one of that cost is unassigned, in which
+// case the last such one.  gt_inds [B, LP]: 0 = background, j + 1 = matched to box j.
 // ---------------------------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(32)
 hungarian_kernel(const float* __restrict__ cost, const float* __restrict__ iou, const int* __restrict__ n_gt, int P, int L,
@@ -138,7 +141,7 @@ hungarian_kernel(const float* __restrict__ cost, const float* __restrict__ iou, 
   for (int i = lane; i < P; i += 32) { gi[i] = 0; mo[i] = 0.f; }
   if (G == 0) return;
   const float* C = cost + ((size_t)b * LP + (size_t)l * P) * Gmax;       // C[i * Gmax + j]
-  const bool tr = G <= P;                  // rows of the solver = ground-truth boxes when there are fewer of them
+  const bool tr = G < P;                   // rows of the solver = ground-truth boxes when there are fewer of them
   const int nr = tr ? G : P, nc = tr ? P : G;
   auto cst = [&](int r, int c) -> double { return tr ? (double)C[(size_t)c * Gmax + r] : (double)C[(size_t)r * Gmax + c]; };
   const int NMAX = max(P, Gmax);
@@ -150,40 +153,47 @@ hungarian_kernel(const float* __restrict__ cost, const float* __restrict__ iou, 
   int* row4col = col4row + NMAX;
   int* SR = row4col + NMAX;
   int* SC = SR + NMAX;
+  int* rem = SC + NMAX;                    // scipy's `remaining`: the unvisited columns, in its scan order
   for (int k = lane; k < NMAX; k += 32) { u[k] = 0.0; v[k] = 0.0; col4row[k] = -1; row4col[k] = -1; }
   __syncwarp();
   const double INF = 1e300;
+  // scan position `it` of cost s (free: unassigned column) beats the best so far: the least cost; among equal costs an
+  // unassigned column, the last one in scan order; else the first one (scipy's sequential `<`, `== && free` rule)
+  auto better = [](double s, int fr, int it, double best, int bfree, int bit) {
+    return s < best || (s == best && (fr > bfree || (fr == bfree && (fr ? it > bit : it < bit))));
+  };
   for (int cur = 0; cur < nr; ++cur) {
     for (int k = lane; k < NMAX; k += 32) { spc[k] = INF; SR[k] = 0; SC[k] = 0; }
+    for (int k = lane; k < nc; k += 32) rem[k] = nc - 1 - k;
     __syncwarp();
     double minVal = 0.0;
-    int i = cur, sink = -1;
+    int i = cur, sink = -1, nrem = nc;
     while (sink < 0) {
       if (lane == 0) SR[i] = 1;
       double best = INF;
-      int bidx = 0x7fffffff, bfree = 0;
+      int bit = -1, bfree = 0;
       const double ui = u[i];
-      for (int j = lane; j < nc; j += 32) {
-        if (SC[j]) continue;
+      for (int it = lane; it < nrem; it += 32) {
+        const int j = rem[it];
         const double r = minVal + cst(i, j) - ui - v[j];
         if (r < spc[j]) { spc[j] = r; path[j] = i; }
         const double s = spc[j];
         const int fr = row4col[j] < 0;
-        // smallest cost; among equal costs prefer an unassigned column, then the smaller index
-        if (s < best || (s == best && (fr > bfree || (fr == bfree && j < bidx)))) { best = s; bidx = j; bfree = fr; }
+        if (better(s, fr, it, best, bfree, bit)) { best = s; bit = it; bfree = fr; }
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
         const double ob = __shfl_xor_sync(0xffffffffu, best, o);
-        const int oi = __shfl_xor_sync(0xffffffffu, bidx, o), of = __shfl_xor_sync(0xffffffffu, bfree, o);
-        if (ob < best || (ob == best && (of > bfree || (of == bfree && oi < bidx)))) { best = ob; bidx = oi; bfree = of; }
+        const int oi = __shfl_xor_sync(0xffffffffu, bit, o), of = __shfl_xor_sync(0xffffffffu, bfree, o);
+        if (better(ob, of, oi, best, bfree, bit)) { best = ob; bit = oi; bfree = of; }
       }
       minVal = best;
-      const int j = bidx;
-      if (j == 0x7fffffff) { sink = -2; break; }              // infeasible (cannot happen with finite costs)
+      if (bit < 0) { sink = -2; break; }                      // infeasible (cannot happen with finite costs)
+      const int j = rem[bit];
       if (row4col[j] < 0) sink = j; else i = row4col[j];
       __syncwarp();
-      if (lane == 0) SC[j] = 1;
+      if (lane == 0) { SC[j] = 1; rem[bit] = rem[nrem - 1]; }
+      --nrem;
       __syncwarp();
     }
     if (sink == -2) break;
@@ -419,7 +429,8 @@ __global__ void loss_finish_kernel(const double* __restrict__ hpart, const doubl
 
 // HeuristicAssigner3D.assign (hungarian_assigner.py:60-91): every ground-truth box claims its nearest prediction (BEV centre
 // distance, + dist_thre when the query's class differs); a prediction claimed twice keeps the nearer box (ties: the earlier
-// box, the reference's strict `<`).  One CTA; P, G small.
+// box, the reference's strict `<`).  As in the reference, a claim must also be nearer than 10000, the distance an
+// unclaimed prediction starts with.  One CTA; P, G small.
 __global__ void __launch_bounds__(256)
 heuristic_assign_kernel(const float* __restrict__ boxes, int nb, int P, const float* __restrict__ gt, const int* __restrict__ gt_labels,
                         int G, const int* __restrict__ query_labels, float dist_thre, long long* __restrict__ gt_inds,
@@ -443,7 +454,7 @@ heuristic_assign_kernel(const float* __restrict__ boxes, int nb, int P, const fl
     for (int g = 0; g < G; ++g) {
       const int i = nearest[g];
       const float d = ndist[g];
-      if (d <= dist_thre && (gt_inds[i] == 0 || d < overlaps[i])) {   // overlaps[] holds the claimed distance for now
+      if (d <= dist_thre && d < (gt_inds[i] == 0 ? 10000.f : overlaps[i])) {   // overlaps[] holds the claimed distance for now
         overlaps[i] = d;
         gt_inds[i] = g + 1;
         labels[i] = (float)gt_labels[g];
@@ -496,7 +507,7 @@ int di_hungarian_f32(const float* cost, const float* iou, const int* n_gt, int B
                      float* max_overlaps, cudaStream_t stream) {
   DI_CHECK_ARG(cost && iou && n_gt && gt_inds && max_overlaps && B > 0 && L > 0 && P > 0 && Gmax > 0, "di_hungarian_f32: bad argument");
   const int nmax = P > Gmax ? P : Gmax;
-  const int smem = nmax * (3 * (int)sizeof(double) + 5 * (int)sizeof(int));
+  const int smem = nmax * (3 * (int)sizeof(double) + 6 * (int)sizeof(int));
   DI_CHECK_ARG(smem <= 200 * 1024, "di_hungarian_f32: problem too large (P=%d, G=%d)", P, Gmax);
   static DiSmemOnce once{};
   if (!di_smem_once(once, hungarian_kernel, 200 * 1024)) {
