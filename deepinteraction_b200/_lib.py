@@ -71,6 +71,7 @@ SIGNATURES = {
     'di_heatmap_nms_f32': [_p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_topk_f32': [_p, _p, _i, _i, _i, _p, _i, _p],
     'di_query_init_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
+    'di_query_init_bwd_f32': [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
     'di_mha_small_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _p],
     'di_mha_small_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _p, _p, _p, _i, _i, _i, _i, _p],
     'di_cross_attn_f32': [_p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
@@ -103,6 +104,8 @@ SIGNATURES = {
     'di_gaussian_heatmap_f32': [_p, _i, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p],
     'di_mmpi_losses_f32': [_p, _p, _ll, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p,
                            _p, _p, _p, _p],
+    'di_mmpi_losses_bwd_f32': [_p, _p, _ll, _i, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p, _p, _p, _p,
+                               _p, _p, _p, _p, _p],
     'di_pred_finish_pp_f32': [_p, _p, _p, _p, _p, _p, _i, _i, _i, _p],
     'di_rcnn_leaders': [_p, _p, _p, _i, _i, _i, _p],
     'di_mha_small_rows_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],

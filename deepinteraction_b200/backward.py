@@ -49,6 +49,16 @@ def _add(a, b):
     return ops.axpy(a.contiguous(), b.contiguous(), _ONE[a.device])
 
 
+_MINUS_ONE = {}
+
+
+def _sub(a, b):
+    """a - b on the device."""
+    if a.device not in _MINUS_ONE:
+        _MINUS_ONE[a.device] = torch.full((1,), -1.0, device=a.device)
+    return ops.axpy(a.contiguous(), b.contiguous(), _MINUS_ONE[a.device])
+
+
 def _bw_pack(pk):
     """Transposed weights for the dX products, built once per pack."""
     if '_bw' not in pk:
@@ -166,9 +176,13 @@ def i2p_backward(i2p_pack, pts_nhwc, img_nhwc, pts_metas, proj, V, in_hw, grad_o
 def conv3x3_wgrad(x_nchw, g_rows, cout):
     """dW [Cout, Cin, 3, 3] and db of a 3x3 convolution: per tap a split-K product of the output gradient with the shifted
     input (dW[co, ci, ky, kx] = sum_p dY[p, co] X[p + (ky - 1, kx - 1), ci])."""
-    x_nhwc = ops.nchw_to_nhwc(x_nchw.contiguous())
+    return _conv3x3_wgrad_nhwc(ops.nchw_to_nhwc(x_nchw.contiguous()), g_rows, cout)
+
+
+def _conv3x3_wgrad_nhwc(x_nhwc, g_rows, cout):
+    """conv3x3_wgrad of a pixel-major input [N, H, W, Cin]."""
     cin = x_nhwc.shape[-1]
-    dw = torch.empty(cout, cin, 3, 3, device=x_nchw.device)
+    dw = torch.empty(cout, cin, 3, 3, device=x_nhwc.device)
     for ky in range(3):
         for kx in range(3):
             xs = ops.shift_map(x_nhwc, ky - 1, kx - 1).view(-1, cin)
@@ -200,11 +214,21 @@ def _shared_conv_backward(g_rows, w_packed, x_nchw):
     (dW [Cout, Cin, 3, 3], db)).  d x = conv3x3(d y, W^T flipped): the packed forward weight [Cout, (ky*3+kx)*Cin + ci]
     becomes the packed weight [Cin, (ky*3+kx)*Cout + co] with the taps flipped, on the device."""
     N, cin, H, W = x_nchw.shape
+    cout = w_packed.shape[0]
+    dx = ops.conv3x3(g_rows.view(N, H, W, cout), _flipped(w_packed), None, cout=cin, x_nhwc=True)
+    return dx, conv3x3_wgrad(x_nchw, g_rows, cout)
+
+
+def _flipped(w_packed, cout=None):
+    """Packed 3x3 weight [Cout, (ky*3+kx)*Cin + ci] -> fold.Weight [Cin, (ky*3+kx)*cout + co] of the transposed convolution,
+    taps flipped, on the device; cout > Cout pads the output channels of the forward with zero rows."""
     w = w_packed.w.detach()
+    co, cin = w.shape[0], w.shape[1] // 9
+    if cout is not None and cout > co:
+        w = torch.cat([w, torch.zeros(cout - co, w.shape[1], device=w.device, dtype=w.dtype)], 0)
     cout = w.shape[0]
     wt = w.view(cout, 3, 3, cin).flip(1, 2).permute(3, 1, 2, 0).reshape(cin, 9 * cout)   # co, ky, kx, ci -> ci, ky', kx', co
-    dx = ops.conv3x3(g_rows.view(N, H, W, cout), fold.Weight(wt.contiguous(), w.device, lazy=True), None, cout=cin, x_nhwc=True)
-    return dx, conv3x3_wgrad(x_nchw, g_rows, cout)
+    return fold.Weight(wt.contiguous(), w.device, lazy=True)
 
 
 def _fuse_bw_pack(lp):
@@ -591,3 +615,215 @@ class ImageRCNNFunction(torch.autograd.Function):
         query, pred, img = ctx.saved_tensors
         r = image_rcnn_backward(ctx.dec, ctx.li, query, pred, img, ctx.img_metas, grad_out)
         return None, None, r['d_query'], None, r['d_img'], None
+
+
+# ---- decoder: prediction heads, heat-map head, query init and the whole base decoder from its loss ---------------------
+def _pred_bw_pack(dec, li, pack):
+    """Transposed weights of a prediction FFN's two dX products and, per head, its row / column ranges in the packed
+    weights (mmpi._pack_pred) with the constants of fold.conv_bn_unfold, built once per pack.  li: index into
+    dec.pred_head, or None for dec.prediction_heads[0]."""
+    pk = dec.pack()
+    holder = pk if li is None else pk['blocks'][li]
+    if '_bw_pred' not in holder:
+        ffn = dec.prediction_heads[0] if li is None else dec.pred_head[li]
+        dev_ = pk['bce'].device
+        heads, r, c = [], 0, 0
+        for h in dec.head_order:
+            seq = getattr(ffn, h)
+            n1, n2 = seq[0].conv.weight.shape[0], seq[1].weight.shape[0]
+            consts = tuple(t.to(device=dev_, dtype=torch.float32) for t in fold.conv_bn_unfold_consts(seq[0].conv, seq[0].bn))
+            heads.append((h, slice(r, r + n1), slice(c, c + n2), consts))
+            r, c = r + n1, c + n2
+        holder['_bw_pred'] = dict(w1=_transposed(pack[0]), w2=_transposed(pack[2]), heads=heads)
+    return holder['_bw_pred']
+
+
+@_precise()
+def pred_head_backward(dec, li, srcs, grad_out):
+    """Backward of a prediction FFN (reference models/utils/decoder_utils.py:498-581; per head ConvBN1d(cin -> 64) + ReLU,
+    Conv1d(64 -> k), BatchNorm in eval mode) as the forward packs it: one [sum 64, cin] layer over every head, then a
+    block-diagonal [NP, sum 64] one.  li: index into dec.pred_head (input cat([query, previous query]), :289), or None for
+    dec.prediction_heads[0] (input the query).  srcs: the input rows [B*P, C] as the forward feeds them; grad_out
+    [B*P, NP]: gradient of the head's output rows (head order, before the forward adds query_pos to the centre, which
+    passes it unchanged).  -> dict(d_srcs = [d src], grads = {name: tensor} for '{h}.0.conv.weight', '{h}.0.bn.weight',
+    '{h}.0.bn.bias', '{h}.1.weight', '{h}.1.bias' of every head h, shaped as in the FFN's state_dict).  The hidden rows are
+    re-run for the ReLU mask; only the diagonal blocks of the second layer's weight gradient are parameters."""
+    pk = dec.pack()
+    pack = pk['pred0'] if li is None else pk['blocks'][li]['pred']
+    bw = _pred_bw_pack(dec, li, pack)
+    srcs = [s.contiguous() for s in srcs]
+    dy = grad_out.contiguous()
+    W1, b1 = pack[0], pack[1]
+    h = dec._mlp(srcs, W1, b1, ops.ACT_RELU)
+    dW2, db2 = _layer_grads(dy, h)
+    dh = ops.relu_bwd(ops.linear([dy], bw['w2']), h)
+    dW1, db1 = _layer_grads(dh, *srcs)
+    dx = ops.linear([dh], bw['w1'])
+    R = {}
+    for name, rows, cols, consts in bw['heads']:
+        dW0, _, dgamma, dbeta = fold.conv_bn_unfold(consts, dW1[rows], db1[rows])
+        R[name + '.0.conv.weight'] = dW0.unsqueeze(-1)
+        R[name + '.0.bn.weight'], R[name + '.0.bn.bias'] = dgamma, dbeta
+        R[name + '.1.weight'] = dW2[cols, rows].unsqueeze(-1)
+        R[name + '.1.bias'] = db2[cols]
+    k, d_srcs = 0, []
+    for s in srcs:
+        d_srcs.append(dx[:, k:k + s.shape[1]].contiguous())
+        k += s.shape[1]
+    return dict(d_srcs=d_srcs, grads=R)
+
+
+def _heat_bw_pack(dec, pk):
+    """Flipped, transposed weights of the two heat-map convolutions (the second padded to 32 output channels, the
+    layout of the loss gradient) and the constants of fold.conv_bn_unfold, built once per pack."""
+    if '_bw_heat' not in pk:
+        seq = dec.heatmap_head_img
+        w0, _, w1, _ = pk['heatmap_head_img']
+        consts = tuple(t.to(device=w0.w.device, dtype=torch.float32) for t in fold.conv_bn_unfold_consts(seq[0].conv, seq[0].bn))
+        pk['_bw_heat'] = dict(w0=_flipped(w0), w1=_flipped(w1, 32), unfold=consts)
+    return pk['_bw_heat']
+
+
+@_precise()
+def heatmap_head_backward(dec, new_pts, grad_out):
+    """Backward of dec.heatmap_head_img (reference deepinteraction_decoder.py:224: ConvBN2d(C -> C, 3x3) + ReLU, Conv2d(C
+    -> K, 3x3), BatchNorm in eval mode).  new_pts [B, Y, X, C] (pixel-major); grad_out [B, Y, X, 32]: gradient of the
+    dense logits, channels K..31 zero (LossMixin.loss_backward); the weight gradient reads its first K channels.  -> dict(d_new_pts [B, Y, X, C], grads = {name: tensor}
+    for '0.conv.weight', '0.bn.weight', '0.bn.bias', '1.weight', '1.bias', shaped as in its state_dict).  The first
+    convolution is re-run for the ReLU mask; input gradients go through the transposed, tap-flipped convolutions."""
+    pk = dec.pack()
+    bw = _heat_bw_pack(dec, pk)
+    B, Y, X, C = new_pts.shape
+    K = dec.heatmap_head_img[1].weight.shape[0]
+    x = new_pts.contiguous()
+    g = grad_out.contiguous()
+    w0, b0, _, _ = pk['heatmap_head_img']
+    h = ops.conv3x3(x, w0, b0, C, True, False, ops.ACT_RELU)
+    dh = ops.relu_bwd(ops.conv3x3(g, bw['w1'], None, cout=C, x_nhwc=True), h)
+    dW1, db1 = _conv3x3_wgrad_nhwc(h, g.view(-1, 32)[:, :K].contiguous(), K)     # the pad channels are no parameters
+    dx = ops.conv3x3(dh, bw['w0'], None, cout=C, x_nhwc=True)
+    dW0, db0 = _conv3x3_wgrad_nhwc(x, dh.view(-1, C), C)
+    dWc, _, dgamma, dbeta = fold.conv_bn_unfold(bw['unfold'], dW0.reshape(C, -1), db0)
+    R = {'0.conv.weight': dWc.view(C, C, 3, 3), '0.bn.weight': dgamma, '0.bn.bias': dbeta, '1.weight': dW1, '1.bias': db1}
+    return dict(d_new_pts=dx, grads=R)
+
+
+def _decoder_checks(dec, pts_conv, new_pts, img):
+    """NotImplementedError before any launch for what decoder_backward does not cover, including what the block
+    backwards reject (_v1_rcnn_block): the maps' shapes and channels."""
+    B, P, C = pts_conv.shape[0], dec.num_proposals, dec.hidden_channel
+    bev = (B, dec.y_size, dec.x_size, C)
+    if (pts_conv.dim() != 4 or tuple(pts_conv.shape) != bev or tuple(new_pts.shape) != bev or img.dim() != 4
+            or img.shape[0] != B * dec.num_views or img.shape[3] != C or P > 512):
+        raise NotImplementedError(f'decoder_backward: pts_conv and new_pts must be [B, {dec.y_size}, {dec.x_size}, {C}] and '
+                                  f'img [B*{dec.num_views}, h, w, {C}], pixel-major (got {tuple(pts_conv.shape)}, '
+                                  f'{tuple(new_pts.shape)}, {tuple(img.shape)})')
+    from .mmpi import DeepInteractionPlusPlusDecoder
+    if isinstance(dec, DeepInteractionPlusPlusDecoder) or any(getattr(b, 'v2', False) for b in dec.decode_head):
+        raise NotImplementedError('decoder_backward covers the base DeepInteractionDecoder only (the V2 RCNN blocks of the '
+                                  '++ decoder have no backward)')
+    if not dec.auxiliary:
+        raise NotImplementedError('decoder_backward needs auxiliary=True (a loss on every layer), as both reference configs')
+    if dec.num_heads != 8 or dec.hidden_channel != 128 or P > 256 or dec.num_classes_heat > 32 or B < 1:
+        raise NotImplementedError('decoder_backward: the gradient kernels take 8 heads x 16 channels, P <= 256 proposals '
+                                  f'and K <= 32 classes (got heads={dec.num_heads}, C={dec.hidden_channel}, P={P}, '
+                                  f'K={dec.num_classes_heat})')
+
+
+def _prefixed(R, prefix, grads):
+    for k, v in grads.items():
+        R[prefix + k] = v
+
+
+@_precise()
+def decoder_backward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_labels_3d, grad_losses=None):
+    """Gradient of the base decoder's losses (reference deepinteraction_decoder.py:201-313 forward, :484-547 loss) with
+    BatchNorm in eval mode (the folded weights of the forward) and dropout off.
+    dec: DeepInteractionDecoder on the GPU with train_cfg; pts_conv, new_pts [B, Y, X, C], img [B*V, h, w, C]: the encoder's
+    outputs (pixel-major, as forward_rows takes them); img_metas; gt_bboxes_3d / gt_labels_3d as dec.loss takes them;
+    grad_losses [2 + 2L] (device): the upstream gradient of the loss dict's values in their order (None = ones: mmdet's
+    sum of every key containing 'loss'; matched_ious takes none).
+    -> dict(losses = dec.loss(...) of this forward, d_pts_conv [B, Y, X, C], d_new_pts [B, Y, X, C], d_img [B*V, h, w, C],
+    grads = {name: tensor} keyed and shaped as dec.state_dict() for every parameter but heatmap_head.* (the heat map the
+    loss reads comes from heatmap_head_img; heatmap_head only ranks proposals, through .detach(), so autograd gives it
+    None)).  Proposals, RoIs, view groups and the assignment are constants, as in the reference.  The prediction rows of
+    queries on no live view take prediction_heads[0]'s rows by selection, so their gradient goes to that head; they
+    carry weight 0 under the on-image mask, so its gradient is exactly zero in the base decoder.  Everything stays on the device, without host synchronisation after
+    the first call of a pack (ground truth and img_metas as the forward and loss take them; boxes given on the device)."""
+    B, P = pts_conv.shape[0], dec.num_proposals
+    _decoder_checks(dec, pts_conv, new_pts, img)
+    pk = dec.pack()
+    dev_ = pts_conv.device
+    pts_conv, new_pts, img = pts_conv.contiguous(), new_pts.contiguous(), img.contiguous()
+    # ---- forward with the values the chain needs: the forward schedule's own kernels, run eagerly
+    proj, aux = (t.pin_memory().to(dev_, non_blocking=True) for t in dec._camera_consts(img_metas))
+    sv = {}
+    r = dec._schedule(pts_conv, new_pts, img, geom.input_hw(img_metas), proj, aux, sv)
+    losses = dec.loss(gt_bboxes_3d, gt_labels_3d, dec._outputs(r, B))
+    d_heat, d_pred = dec.loss_backward(grad_losses)
+    # ---- MMPI layers in reverse: pred_head[l] reads [q_{l+1} | q_l]; block l maps q_l to q_{l+1} with the RoIs of the
+    # previous layer's (detached) predictions
+    qs = [sv['query_feat1']] + sv['layer_query']
+    R = {}
+    dq, d_img, d_new_pts, d_first = None, None, None, None
+    wins = iter(reversed(r['wins']))
+    for li in reversed(range(len(pk['blocks']))):
+        bp = pk['blocks'][li]
+        d_rows = d_pred[li]
+        if bp['image']:
+            # rows on no live view are prediction_heads[0]'s rows, selected (pred_finish): their gradient goes there
+            d_head = ops.rows_finish(d_rows, zero_if_neg=next(wins))
+            d_first = _add(d_first, _sub(d_rows, d_head))
+            d_rows = d_head
+        ph = pred_head_backward(dec, li, [qs[li + 1], qs[li]], d_rows)
+        _prefixed(R, 'pred_head.%d.' % li, ph['grads'])
+        pred_in = r['preds'][li - 1] if li > 0 else sv['first_res']
+        d_out = _add(dq, ph['d_srcs'][0])
+        if bp['image']:
+            d_q, d_maps, g = _v1_rcnn_backward(dec, bp, B, P, qs[li], pred_in, img, img_metas, d_out)
+            d_img = _add(d_img, d_maps)
+        else:
+            d_q, d_maps, g = _v1_rcnn_backward(dec, bp, B, P, qs[li], pred_in, new_pts, None, d_out)
+            d_new_pts = _add(d_new_pts, d_maps)
+        _prefixed(R, 'decode_head.%d.' % li, g)
+        dq = _add(d_q, ph['d_srcs'][1])
+    # prediction_heads[0] reads the layer's output q1 and feeds the fallback rows (its RoIs are constants).  Under the
+    # on-image mask those rows carry weight 0, so this is exactly zero in the base decoder; it is computed all the same.
+    pf = pred_head_backward(dec, None, [qs[0]], d_first if d_first is not None else torch.zeros_like(d_pred[0]))
+    _prefixed(R, 'prediction_heads.0.', pf['grads'])
+    dq = _add(dq, pf['d_srcs'][0])
+    # ---- transformer layer, query init, heat-map head
+    rl = decoder_layer_backward(dec, sv['query_feat0'], sv['query_pos0'], pts_conv, dq)
+    _prefixed(R, 'decoder.0.', rl['grads'])
+    d_pts_conv = rl['d_bev'].contiguous()
+    d_wce, d_bce = ops.query_init_bwd(rl['d_query'], sv['top'], r['labels'], d_pts_conv.view(B, -1, dec.hidden_channel),
+                                      dec.num_classes_heat)
+    R['class_encoding.weight'], R['class_encoding.bias'] = d_wce.unsqueeze(-1), d_bce
+    hh = heatmap_head_backward(dec, new_pts, d_heat)
+    _prefixed(R, 'heatmap_head_img.', hh['grads'])
+    d_new_pts = _add(d_new_pts, hh['d_new_pts'])
+    if d_img is None:
+        d_img = torch.zeros_like(img)
+    return dict(losses=losses, d_pts_conv=d_pts_conv, d_new_pts=d_new_pts, d_img=d_img, grads=R)
+
+
+class DecoderLossFunction(torch.autograd.Function):
+    """autograd wrapper: the base decoder's summed loss (mmdet's sum of every loss key) from the encoder outputs
+    pts_conv, new_pts [B, Y, X, C] and img [B*V, h, w, C]; backward -> (d_pts_conv, d_new_pts, d_img) through
+    decoder_backward.  Parameter gradients are returned by decoder_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_labels_3d):
+        _decoder_checks(dec, pts_conv, new_pts, img)
+        ctx.dec, ctx.args = dec, (img_metas, gt_bboxes_3d, gt_labels_3d)
+        ctx.save_for_backward(pts_conv, new_pts, img)
+        losses = dec.loss(gt_bboxes_3d, gt_labels_3d, dec.forward_nhwc(pts_conv, new_pts, img, img_metas))
+        return torch.stack([v for k, v in losses.items() if 'loss' in k]).sum()
+
+    @staticmethod
+    def backward(ctx, grad):
+        pts_conv, new_pts, img = ctx.saved_tensors
+        L = len(ctx.dec.decode_head)
+        g = grad.reshape(1).float().expand(2 + 2 * L).contiguous()
+        r = decoder_backward(ctx.dec, pts_conv, new_pts, img, *ctx.args, grad_losses=g)
+        return None, r['d_pts_conv'], r['d_new_pts'], r['d_img'], None, None, None

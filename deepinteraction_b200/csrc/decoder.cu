@@ -230,6 +230,43 @@ __global__ void query_init_kernel(const float* __restrict__ feat, const int* __r
     qscore[((size_t)b * K + c) * P + qi] = heat[((size_t)b * K + c) * HW + pix];
 }
 
+// Backward of the feature gather: d_feat[b, pix, :] += the d qfeat rows of the proposals at pix, in proposal order.  One
+// CTA per proposal; the first proposal at a pixel owns it and sums all of them, the others return (no atomics).
+__global__ void __launch_bounds__(128)
+query_init_bwd_feat_kernel(const float* __restrict__ dq, const int* __restrict__ top, float* __restrict__ d_feat, int HW,
+                           int C, int P) {
+  extern __shared__ int s_pix[];
+  const int b = blockIdx.y, qi = blockIdx.x;
+  for (int j = threadIdx.x; j < P; j += blockDim.x) s_pix[j] = top[b * P + j] % HW;
+  __syncthreads();
+  const int pix = s_pix[qi];
+  int shared_earlier = 0;
+  for (int j = threadIdx.x; j < qi; j += blockDim.x) shared_earlier |= s_pix[j] == pix;
+  if (__syncthreads_or(shared_earlier)) return;
+  float* dst = d_feat + ((size_t)b * HW + pix) * C;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float s = dst[c];
+    for (int j = qi; j < P; ++j)
+      if (s_pix[j] == pix) s += dq[((size_t)b * P + j) * C + c];
+    dst[c] = s;
+  }
+}
+
+// Backward of the class encoding (Conv1d(K, C, 1) on the one-hot labels): block k < K -> d_w[c, k] = sum of the d qfeat
+// rows with label k; block K -> d_b[c] = sum of all rows.  Rows in order, one thread per output.
+__global__ void __launch_bounds__(128)
+query_init_bwd_class_kernel(const float* __restrict__ dq, const int* __restrict__ labels, float* __restrict__ d_w,
+                            float* __restrict__ d_b, int M, int C, int K) {
+  const int k = blockIdx.x;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float s = 0.f;
+    for (int r = 0; r < M; ++r)
+      if (k == K || labels[r] == k) s += dq[(size_t)r * C + c];
+    if (k == K) d_b[c] = s;
+    else d_w[(size_t)c * K + k] = s;
+  }
+}
+
 // ------------------------------------------------------------------------------------------------
 // Small multi-head attention among the P queries of one sample (self-attention of the transformer
 // layer and of the RCNN blocks).  One warp per (query, head).  Optional group mask: key j is visible to
@@ -1758,6 +1795,16 @@ int di_query_init_f32(const float* feat, const int* top, const float* heat, cons
   DI_CHECK_ARG(feat && top && heat && wce_t && bce && qfeat && qpos && labels && qscore, "di_query_init_f32: null pointer");
   query_init_kernel<<<B * P, 128, 0, stream>>>(feat, top, heat, wce_t, bce, qfeat, qpos, labels, qscore, HW, W, C, K, P);
   DI_CHECK_LAUNCH("di_query_init_f32");
+  return DI_OK;
+}
+
+int di_query_init_bwd_f32(const float* dq, const int* top, const int* labels, float* d_feat, float* d_wce, float* d_bce, int B,
+                          int HW, int C, int K, int P, cudaStream_t stream) {
+  DI_CHECK_ARG(dq && top && labels && d_feat && d_wce && d_bce && B > 0 && HW > 0 && C > 0 && K > 0 && P > 0 && P <= 8192,
+               "di_query_init_bwd_f32: bad argument");
+  query_init_bwd_feat_kernel<<<dim3(P, B), 128, P * sizeof(int), stream>>>(dq, top, d_feat, HW, C, P);
+  query_init_bwd_class_kernel<<<K + 1, 128, 0, stream>>>(dq, labels, d_wce, d_bce, B * P, C, K);
+  DI_CHECK_LAUNCH("di_query_init_bwd_f32");
   return DI_OK;
 }
 

@@ -427,6 +427,106 @@ __global__ void loss_finish_kernel(const double* __restrict__ hpart, const doubl
   out[1 + 2 * L] = (float)(m / (double)B);
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// loss gradients: the avg factors come from the device (no .item()), one thread per output element, no atomics
+// ---------------------------------------------------------------------------------------------------------------------
+// cnt[blk] = #(target == 1) of the block's grid-stride share, as heatmap_loss_kernel counts it
+__global__ void __launch_bounds__(256)
+heat_count_kernel(const float* __restrict__ target, long long n, double* __restrict__ cnt) {
+  __shared__ double red[8];
+  double c = 0.0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    c += target[i] == 1.f ? 1.0 : 0.0;
+  c = block_sum(c, red);
+  if (threadIdx.x == 0) cnt[blockIdx.x] = c;
+}
+
+// scale[0] = g[0] w_heat / max(#ones, 1); scale[1 + 2 l] = g[1 + 2 l] w_cls / max(num_pos_l, 1); scale[2 + 2 l] likewise
+// with w_box: d loss / d (one weighted term) of every loss, as loss_finish_kernel divides
+__global__ void loss_bwd_scale_kernel(const double* __restrict__ hcnt, int nh, const float* __restrict__ num_pos, int L,
+                                      const float* __restrict__ grad, float w_heat, float w_cls, float w_box,
+                                      float* __restrict__ scale) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  double c = 0.0;
+  for (int k = 0; k < nh; ++k) c += hcnt[k];
+  scale[0] = (float)((double)grad[0] * (double)w_heat / fmax(c, 1.0));
+  for (int l = 0; l < L; ++l) {
+    const double af = fmax((double)num_pos[l], 1.0);
+    scale[1 + 2 * l] = (float)((double)grad[1 + 2 * l] * (double)w_cls / af);
+    scale[2 + 2 * l] = (float)((double)grad[2 + 2 * l] * (double)w_box / af);
+  }
+}
+
+// d GaussianFocalLoss(clip_sigmoid(logit)) / d logit, written pixel-major [B, HW, 32] (channels K..31 = 0): the input
+// layout of the transposed 3x3 convolution.  clip_sigmoid's clamp passes the gradient by torch's rule (zero strictly
+// outside [1e-4, 1 - 1e-4]); the sigmoid's derivative is taken at the unclamped p.  One thread per 4 channels of a pixel.
+__global__ void __launch_bounds__(256)
+heatmap_loss_bwd_kernel(const float* __restrict__ logit, const float* __restrict__ target, int B, int K, int HW, float alpha,
+                        float gamma, const float* __restrict__ scale, float* __restrict__ d_out) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= (long long)B * HW * 8) return;
+  const int c4 = (int)(t & 7);
+  const long long bp = t >> 3;
+  const int b = (int)(bp / HW), pix = (int)(bp - (long long)b * HW);
+  const float s = scale[0];
+  float d[4];
+#pragma unroll
+  for (int u = 0; u < 4; ++u) {
+    const int c = c4 * 4 + u;
+    d[u] = 0.f;
+    if (c >= K) continue;
+    const size_t i = ((size_t)b * K + c) * HW + pix;
+    const float p = 1.f / (1.f + expf(-logit[i]));
+    if (!(p >= 1e-4f && p <= 1.f - 1e-4f)) continue;
+    const float tg = target[i];
+    float g = 0.f;
+    if (tg == 1.f)
+      g = -powf(1.f - p, alpha) / (p + 1e-12f) + alpha * logf(p + 1e-12f) * powf(1.f - p, alpha - 1.f);
+    else
+      g = (powf(p, alpha) / (1.f - p + 1e-12f) - alpha * logf(1.f - p + 1e-12f) * powf(p, alpha - 1.f)) * powf(1.f - tg, gamma);
+    d[u] = g * (p * (1.f - p)) * s;
+  }
+  reinterpret_cast<float4*>(d_out)[t] = make_float4(d[0], d[1], d[2], d[3]);
+}
+
+// d layer losses / d prediction rows [L, B*P, NP] in head order (centre, height, dim, rot[, vel], heatmap): the box-code
+// columns take sign(pred - target) x bbox weight x code weight (0 at equality, as torch's abs), the K class columns
+// mmcv's closed-form sigmoid focal gradient (FLT_MIN inside the logs only) x label weight.  A zero weight writes 0.
+__global__ void __launch_bounds__(256)
+layer_loss_bwd_kernel(const float* __restrict__ score, LayerLossParams lp, const long long* __restrict__ labels,
+                      const long long* __restrict__ label_w, const float* __restrict__ bbox_t, const float* __restrict__ bbox_w,
+                      const float* __restrict__ scale, float* __restrict__ d_pred) {
+  const int NP = lp.code + lp.K, LP = lp.L * lp.P;
+  const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= (long long)lp.L * lp.B * lp.P * NP) return;
+  const int j = (int)(e % NP);
+  const int r = (int)(e / NP);                                  // l * B*P + b * P + i
+  const int l = r / (lp.B * lp.P), bi = r - l * (lp.B * lp.P), b = bi / lp.P, i = bi - b * lp.P, q = l * lp.P + i;
+  const size_t t = (size_t)b * LP + q;
+  float d = 0.f;
+  if (j < lp.code) {
+    const float w = bbox_w[t * lp.code + j] * lp.code_w[j];
+    if (w != 0.f) {
+      const float* src = j < 2 ? lp.center + ((size_t)b * 2 + j) * LP : j == 2 ? lp.height + (size_t)b * LP
+                       : j < 6 ? lp.dim + ((size_t)b * 3 + (j - 3)) * LP : j < 8 ? lp.rot + ((size_t)b * 2 + (j - 6)) * LP
+                       : lp.vel + ((size_t)b * 2 + (j - 8)) * LP;
+      const float v = src[q] - bbox_t[t * lp.code + j];
+      d = (v > 0.f ? 1.f : v < 0.f ? -1.f : 0.f) * w * scale[2 + 2 * l];
+    }
+  } else {
+    const float w = (float)label_w[t];
+    if (w != 0.f) {
+      const int c = j - lp.code;
+      const float p = 1.f / (1.f + expf(-score[((size_t)b * lp.K + c) * LP + q]));
+      const float g = labels[t] == c
+          ? -lp.alpha * powf(1.f - p, lp.gamma) * (1.f - p - lp.gamma * p * logf(fmaxf(p, 1.17549435e-38f)))
+          : -(1.f - lp.alpha) * powf(p, lp.gamma) * (lp.gamma * (1.f - p) * logf(fmaxf(1.f - p, 1.17549435e-38f)) - p);
+      d = g * w * scale[1 + 2 * l];
+    }
+  }
+  d_pred[e] = d;
+}
+
 // HeuristicAssigner3D.assign (hungarian_assigner.py:60-91): every ground-truth box claims its nearest prediction (BEV centre
 // distance, + dist_thre when the query's class differs); a prediction claimed twice keeps the nearer box (ties: the earlier
 // box, the reference's strict `<`).  As in the reference, a claim must also be nearer than 10000, the distance an
@@ -573,6 +673,38 @@ int di_mmpi_losses_f32(const float* dense_logit, const float* heat_target, long 
   loss_finish_kernel<<<1, 32, 0, stream>>>(hpart, hcnt, NH, lpart, NL, num_pos, iou_sum, pos_cnt, L, B, weights3[0], weights3[1],
                                           weights3[2], out);
   DI_CHECK_LAUNCH("di_mmpi_losses_f32");
+  return DI_OK;
+}
+
+// The inputs of di_mmpi_losses_f32 (dense logits / targets [B, K, Y, X] with HW = Y * X), grad [2 + 2 L] (device): the
+// upstream gradient of each output (the last, matched_ious, takes none).  -> d_heat [B, HW, 32] (pixel-major, channels
+// K..31 written as 0), d_pred [L, B*P, code + K] (head order).  work: double [2 * 256 + L * 2 * 64], as the forward's.
+int di_mmpi_losses_bwd_f32(const float* dense_logit, const float* heat_target, long long n_heat, int HW, const float* score,
+                           const float* center, const float* height, const float* dim, const float* rot, const float* vel,
+                           const long long* labels, const long long* label_w, const float* bbox_t, const float* bbox_w,
+                           const float* num_pos, int B, int K, int L, int P, int code, const float* code_w, const float* focal2,
+                           const float* gfl2, const float* weights3, const float* grad, double* work, float* d_heat,
+                           float* d_pred, cudaStream_t stream) {
+  DI_CHECK_ARG(dense_logit && heat_target && score && center && height && dim && rot && labels && label_w && bbox_t && bbox_w &&
+               num_pos && code_w && focal2 && gfl2 && weights3 && grad && work && d_heat && d_pred && B > 0 && L > 0 && P > 0 &&
+               HW > 0 && K > 0 && K <= 32 && n_heat == (long long)B * K * HW && (code == 8 || (code == 10 && vel)),
+               "di_mmpi_losses_bwd_f32: bad argument");
+  const int NH = 256;
+  double* hcnt = work;
+  float* scale = reinterpret_cast<float*>(work + NH);
+  heat_count_kernel<<<NH, 256, 0, stream>>>(heat_target, n_heat, hcnt);
+  loss_bwd_scale_kernel<<<1, 32, 0, stream>>>(hcnt, NH, num_pos, L, grad, weights3[0], weights3[1], weights3[2], scale);
+  const long long nq = (long long)B * HW * 8;
+  heatmap_loss_bwd_kernel<<<(unsigned)((nq + 255) / 256), 256, 0, stream>>>(dense_logit, heat_target, B, K, HW, gfl2[0], gfl2[1],
+                                                                           scale, d_heat);
+  LayerLossParams lp;
+  lp.center = center; lp.height = height; lp.dim = dim; lp.rot = rot; lp.vel = vel;
+  for (int c = 0; c < 10; ++c) lp.code_w[c] = c < code ? code_w[c] : 0.f;
+  lp.gamma = focal2[0]; lp.alpha = focal2[1];
+  lp.K = K; lp.P = P; lp.L = L; lp.B = B; lp.code = code;
+  const long long ne = (long long)L * B * P * (code + K);
+  layer_loss_bwd_kernel<<<(unsigned)((ne + 255) / 256), 256, 0, stream>>>(score, lp, labels, label_w, bbox_t, bbox_w, scale, d_pred);
+  DI_CHECK_LAUNCH("di_mmpi_losses_bwd_f32");
   return DI_OK;
 }
 

@@ -116,11 +116,26 @@ def decoder_layer_unfold_consts(layer, num_heads, device, dtype=torch.float32):
     u = dict(C=C, s=s, qscale=torch.cat([torch.full((C,), s, dtype=torch.float64), torch.ones(2 * C, dtype=torch.float64)]))
     for name in ('self_posembed', 'cross_posembed'):
         seq = getattr(layer, name).position_embedding_head
-        conv, bn = seq[0], seq[1]
-        W0 = _d(conv.weight).reshape(conv.weight.shape[0], -1)
-        u[name] = (W0, _d(conv.bias) - _d(bn.running_mean), 1.0 / torch.sqrt(_d(bn.running_var) + bn.eps), _d(bn.weight))
+        u[name] = conv_bn_unfold_consts(seq[0], seq[1])
     cast = lambda t: t.to(device=device, dtype=dtype) if torch.is_tensor(t) else t
     return {k: (tuple(cast(x) for x in v) if isinstance(v, tuple) else cast(v)) for k, v in u.items()}
+
+
+def conv_bn_unfold_consts(conv, bn):
+    """Constants of conv_bn_unfold for one convolution + BatchNorm (eval) pair, float64 on the host: the convolution's weight
+    as [Cout, Cin*k*k], its bias (0 without one) minus the BN running mean, the BN 1 / sqrt(var + eps) and gamma."""
+    W0 = _d(conv.weight).reshape(conv.weight.shape[0], -1)
+    b0 = _d(conv.bias) if conv.bias is not None else torch.zeros(W0.shape[0], dtype=torch.float64)
+    return W0, b0 - _d(bn.running_mean), 1.0 / torch.sqrt(_d(bn.running_var) + bn.eps), _d(bn.weight)
+
+
+def conv_bn_unfold(consts, dW1, db1):
+    """Chain rule of the conv + BN fold W1 = W0 sc, b1 = (b0 - mean) sc + beta, sc = gamma / sqrt(var + eps), from the
+    gradients of the folded (W1 [Cout, Cin*k*k], b1) -> (d W0, d b0, d gamma, d beta).  consts: conv_bn_unfold_consts
+    (cast where the gradients are)."""
+    W0, b0m, inv, gamma = consts
+    sc = gamma * inv
+    return dW1 * sc[:, None], db1 * sc, ((dW1 * W0).sum(1) + db1 * b0m) * inv, db1
 
 
 def decoder_layer_unfold(u, g):
@@ -142,13 +157,12 @@ def decoder_layer_unfold(u, g):
     out['multihead_attn.in_proj_bias'] = torch.cat([dbq * s, dbkv])
     for name in ('self_posembed', 'cross_posembed'):
         dW1, db1, dW2, db2 = g[name]
-        W0, b0m, inv, gamma = u[name]
-        sc = gamma * inv
         pre = name + '.position_embedding_head.'
-        out[pre + '0.weight'] = (dW1 * sc[:, None]).unsqueeze(-1)
-        out[pre + '0.bias'] = db1 * sc
-        out[pre + '1.weight'] = ((dW1 * W0).sum(1) + db1 * b0m) * inv
-        out[pre + '1.bias'] = db1
+        dW0, db0, dgamma, dbeta = conv_bn_unfold(u[name], dW1, db1)
+        out[pre + '0.weight'] = dW0.unsqueeze(-1)
+        out[pre + '0.bias'] = db0
+        out[pre + '1.weight'] = dgamma
+        out[pre + '1.bias'] = dbeta
         out[pre + '3.weight'] = dW2.unsqueeze(-1)
         out[pre + '3.bias'] = db2
     return out

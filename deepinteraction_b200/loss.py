@@ -7,7 +7,9 @@ Reference: projects/mmdet3d_plugin/core/bbox/assigners/hungarian_assigner.py (BB
 models/dense_heads/deepinteraction_decoder.py get_targets :315-353, get_targets_single :355-482, loss :484-547
 (deepinteractionplusplus_decoder.py:513-514 for the ++ mask rule).  The reference copies every cost matrix to the CPU
 and calls scipy.optimize.linear_sum_assignment once per layer and sample; here all (sample, layer) problems are solved by
-one kernel launch (di_hungarian_f32).  Forward values only -- gradients are outside this repository's scope.
+one kernel launch (di_hungarian_f32).  LossMixin.loss_backward gives the gradient of the three losses with respect to
+the dense heat-map logits and the prediction rows (di_mmpi_losses_bwd_f32); backward.decoder_backward chains it through
+the whole base decoder.
 
 The classes below carry the names the reference registers (MATCH_COST / BBOX_ASSIGNERS), so `train_cfg.assigner` of
 Fusion_0075_*.py builds unchanged; the cost objects are parameter holders (the arithmetic is fused in
@@ -60,23 +62,38 @@ def _f(vals):
     return (ctypes.c_float * len(vals))(*[float(v) for v in vals])
 
 
+def _to_device(t, device):
+    """Host tensor -> device through pinned memory, without a host synchronisation (a pageable source makes the copy
+    synchronous)."""
+    return t.pin_memory().to(device, non_blocking=True) if torch.device(device).type == 'cuda' else t.to(device)
+
+
 def pad_gt(gt_boxes, gt_labels, device):
-    """list of (G_b, nb) boxes / (G_b,) labels -> padded [B, Gmax, nb] fp32, [B, Gmax] int32, counts [B] int32."""
+    """list of (G_b, nb) boxes / (G_b,) labels -> padded [B, Gmax, nb] fp32, [B, Gmax] int32, counts [B] int32.  Boxes
+    already on the device are padded there; no host synchronisation either way."""
     B = len(gt_boxes)
     nb = gt_boxes[0].shape[-1]
     G = max(1, max(int(b.shape[0]) for b in gt_boxes))
-    boxes = torch.zeros(B, G, nb, dtype=torch.float32)
-    labels = torch.zeros(B, G, dtype=torch.int32)
-    counts = torch.tensor([int(b.shape[0]) for b in gt_boxes], dtype=torch.int32)
     on_dev = all(b.is_cuda for b in gt_boxes)
-    if on_dev:
-        boxes, labels = boxes.to(device), labels.to(device)
+    boxes = torch.zeros(B, G, nb, dtype=torch.float32, device=device if on_dev else 'cpu')
+    labels = torch.zeros(B, G, dtype=torch.int32, device=device if on_dev else 'cpu')
+    counts = torch.tensor([int(b.shape[0]) for b in gt_boxes], dtype=torch.int32)
     for i, (b, l) in enumerate(zip(gt_boxes, gt_labels)):
         n = int(b.shape[0])
         if n:
             boxes[i, :n] = b.to(boxes.device, torch.float32)
             labels[i, :n] = l.to(labels.device, torch.int32)
-    return boxes.to(device), labels.to(device), counts.to(device)
+    if not on_dev:
+        boxes, labels = _to_device(boxes, device), _to_device(labels, device)
+    return boxes, labels, _to_device(counts, device)
+
+
+def losses_bwd_bytes(B, K, HW, L, P, code):
+    """Algorithmic traffic of di_mmpi_losses_bwd_f32: the dense logits and targets read twice (count, gradient), the
+    [B, HW, 32] heat-map gradient written; per prediction row its K + code predictions, label and weight (int64), box
+    targets and weights read, its gradient row written."""
+    rows = B * L * P
+    return 4 * (2 * 2 * B * K * HW + B * HW * 32) + rows * (4 * (K + code) + 16 + 8 * code + 4 * (K + code))
 
 
 class HungarianAssigner3D:
@@ -251,4 +268,37 @@ class LossMixin:
             res[f'layer_{l}_loss_bbox'] = out[2 + 2 * l]
         res['matched_ious'] = out[1 + 2 * L]
         self._last_targets = t
+        self._last_dense = dense
         return res
+
+    def loss_backward(self, grad=None):
+        """Gradient of the losses of the last `loss` call (its targets and inputs; the assignment, targets and avg factors
+        are constants) for the upstream gradient grad [2 + 2 L] of its outputs in their order (device; None = ones, the
+        gradient of mmdet's sum of every loss key; the matched_ious entry takes none).
+        -> (d dense heat-map logits [B, Y, X, 32] pixel-major, channels K..31 zero; d prediction rows [L, B*P, NP] in head
+        order), on the device without a host round trip."""
+        t, dense = self._last_targets, self._last_dense
+        heat, rot, dim, center, height, vel = t['tensors']
+        B, K, LP = heat.shape
+        L, P = t['L'], self.num_proposals
+        dev = heat.device
+        _, _, Y, X = dense.shape
+        if grad is None:
+            grad = torch.ones(2 + 2 * L, device=dev, dtype=torch.float32)
+        grad = grad.to(torch.float32).contiguous()
+        assert grad.shape == (2 + 2 * L,) and grad.is_cuda
+        cw = self.train_cfg.get('code_weights', None)
+        code = self.bbox_coder.code_size
+        lc, lb, lh = self._loss_cfg['cls'], self._loss_cfg['bbox'], self._loss_cfg['heat']
+        work = torch.empty(2 * 256 + L * 2 * 64, device=dev, dtype=torch.float64)
+        d_heat = torch.empty(B, Y, X, 32, device=dev, dtype=torch.float32)
+        d_pred = torch.empty(L, B * P, code + K, device=dev, dtype=torch.float32)
+        ops._call('di_mmpi_losses_bwd_f32', ops._ptr(dense), ops._ptr(t['heatmap']), dense.numel(), Y * X, ops._ptr(heat),
+                  ops._ptr(center), ops._ptr(height), ops._ptr(dim), ops._ptr(rot), ops._ptr(vel), ops._ptr(t['labels']),
+                  ops._ptr(t['label_weights']), ops._ptr(t['bbox_targets']), ops._ptr(t['bbox_weights']), ops._ptr(t['num_pos']),
+                  B, K, L, P, code, _f(list(cw) + [0.0] * (10 - len(cw))), _f([lc.get('gamma', 2.0), lc.get('alpha', 0.25)]),
+                  _f([lh.get('alpha', 2.0), lh.get('gamma', 4.0)]),
+                  _f([lh.get('loss_weight', 1.0), lc.get('loss_weight', 1.0), lb.get('loss_weight', 1.0)]), ops._ptr(grad),
+                  ops._ptr(work), ops._ptr(d_heat), ops._ptr(d_pred), ops._stream(), launches=4,
+                  nbytes=losses_bwd_bytes(B, K, Y * X, L, P, code))
+        return d_heat, d_pred

@@ -589,7 +589,11 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
 
     def forward_nhwc(self, pts_conv, new_pts, img, img_metas, debug=None):
         r = self.forward_rows(pts_conv, new_pts, img, img_metas, debug)
-        B, P = pts_conv.shape[0], self.num_proposals
+        return self._outputs(r, pts_conv.shape[0])
+
+    def _outputs(self, r, B):
+        """forward_rows' result -> the reference's [[dict]] output; sets query_labels and on_the_image_mask."""
+        P = self.num_proposals
         self.query_labels = r['labels'].long()
         if r['keeps']:                                            # ++: one cumulative mask per layer (:295-299)
             self.on_the_image_mask = [(k.view(B, P) != 0) for k in r['keeps']]

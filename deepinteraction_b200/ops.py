@@ -482,6 +482,20 @@ def query_init(feat_nhwc, top, heat, wce_t, bce, W):
     return qfeat, qpos, labels, qscore
 
 
+def query_init_bwd(dq, top, labels, d_feat, K):
+    """Backward of query_init's rows q0 = feat[b, pix] + class encoding: adds the dq [B*P, C] rows into d_feat [B, HW, C]
+    in place at the selected pixels -> (d class_encoding.weight [C, K], d bias [C])."""
+    B, HW, C = d_feat.shape
+    P = top.shape[1]
+    assert dq.is_contiguous() and d_feat.is_contiguous() and top.is_contiguous() and labels.is_contiguous()
+    assert dq.shape == (B * P, C) and top.dtype == torch.int32 and labels.dtype == torch.int32
+    d_w = torch.empty(C, K, device=dq.device, dtype=torch.float32)
+    d_b = torch.empty(C, device=dq.device, dtype=torch.float32)
+    _call('di_query_init_bwd_f32', _ptr(_f32(dq)), _ptr(top), _ptr(labels), _ptr(_f32(d_feat)), _ptr(d_w), _ptr(d_b), B, HW,
+          C, K, P, _stream(), nbytes=4 * (3 * B * P * C + K * C), launches=2)
+    return d_w, d_b
+
+
 def mha_small(q, k, v, B, P, heads, onbits=None, win=None):
     C = q.shape[1]
     out = torch.empty(B * P, C, device=q.device, dtype=torch.float32)

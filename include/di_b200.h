@@ -249,6 +249,11 @@ int di_topk_f32(const float* scores, int* idx, int B, int n, int k, void* work, 
 int di_query_init_f32(const float* feat, const int* top, const float* heat, const float* wce_t, const float* bce,
                       float* qfeat, float* qpos, int* labels, float* qscore, int B, int HW, int W, int C, int K, int P,
                       cudaStream_t stream);
+/* its backward (:245-251, q0 = feat[b, pix] + class_encoding(one_hot(label))): dq [B*P, C] -> d_feat [B, HW, C] += the dq
+ * rows at the selected pixels (proposals sharing a pixel summed in proposal order; other rows untouched), d_wce [C, K]
+ * (class_encoding.weight [C, K, 1]) and d_bce [C] written, rows summed in order.  No atomics; P <= 8192. */
+int di_query_init_bwd_f32(const float* dq, const int* top, const int* labels, float* d_feat, float* d_wce, float* d_bce, int B,
+                          int HW, int C, int K, int P, cudaStream_t stream);
 /* self-attention among the queries of a sample (models/utils/decoder_utils.py:95-99, :745, :826) */
 int di_mha_small_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, float* out, int ldo,
                      const int* onbits, const int* win, int B, int P, int heads, int head_dim, cudaStream_t stream);
@@ -352,6 +357,16 @@ int di_mmpi_losses_f32(const float* dense_logit, const float* heat_target, long 
                        const float* num_pos, const float* iou_sum, const int* pos_cnt, int B, int K, int L, int P, int code,
                        const float* code_w, const float* focal2, const float* gfl2, const float* weights3, double* work,
                        float* out, cudaStream_t stream);
+/* its gradient for upstream grad [2 + 2 L] (device) on the outputs: d_heat [B, HW, 32] d loss / d dense logit, pixel-major,
+ * channels K..31 zero (clip_sigmoid's clamp passes the gradient on [1e-4, 1 - 1e-4]); d_pred [L, B*P, code + K] d loss /
+ * d prediction rows in head order (L1: sign, 0 at equality; focal: mmcv's closed form; rows of zero weight written 0).
+ * Avg factors from the device; one thread per output element, no atomics.  work: double [2 * 256 + L * 2 * 64]. */
+int di_mmpi_losses_bwd_f32(const float* dense_logit, const float* heat_target, long long n_heat, int HW, const float* score,
+                           const float* center, const float* height, const float* dim, const float* rot, const float* vel,
+                           const long long* labels, const long long* label_w, const float* bbox_t, const float* bbox_w,
+                           const float* num_pos, int B, int K, int L, int P, int code, const float* code_w, const float* focal2,
+                           const float* gfl2, const float* weights3, const float* grad, double* work, float* d_heat,
+                           float* d_pred, cudaStream_t stream);
 
 /* ---- backward of the window attention (SURVEY.md 8(b) `di_lcab_backward`; host composition: deepinteraction_b200/backward.py)
  * Pixel-major maps [N*H*W, ld]; tap j = (dy + r) * ks + (dx + r) (locatt_ops/similar.cu:15-17).

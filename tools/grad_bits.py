@@ -5,7 +5,7 @@
     python tools/grad_bits.py --compare DIR_A DIR_B [--spread DIR_A2]
 
 From fixed seeds: lcab_backward (self and cross attention), LCABTrain forward + backward, decoder_layer_backward,
-point_rcnn_backward and image_rcnn_backward (base shapes, batch 2) run on deterministic kernels, so the SHA-256 of every
+point_rcnn_backward, image_rcnn_backward and decoder_backward (base shapes, batch 2) run on deterministic kernels, so the SHA-256 of every
 tensor they return is written and --compare asks the two runs to agree on every hash both have (a version without one of
 the functions is compared on the others).  encoder_backward and encoder_train_step pass through
 di_i2p_attend_bwd_f32 and di_bev_sample_bwd_f32, which accumulate with atomicAdd and differ in the last bits from run to
@@ -84,6 +84,11 @@ def decoder_cases(d):
         img, metas, pred_img = image_inputs(m, B, g, d)
         for li in (0, 2):
             yield f'image_rcnn_backward.{li}', backward.image_rcnn_backward(m, li, query, pred_img, img, metas, grad)
+    if hasattr(backward, 'decoder_backward'):
+        from tools.bench_decoder_bwd import frame, train_decoder
+        mt = train_decoder()
+        r = backward.decoder_backward(mt, *frame(mt, B, g, d))
+        yield 'decoder_backward', {k: v for k, v in r.items() if k != 'losses'}
 
 
 def encoder_cases(d):
