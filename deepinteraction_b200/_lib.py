@@ -111,6 +111,11 @@ SIGNATURES = {
     'di_mha_small_rows_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_take_rows_f32': [_p, _i, _p, _p, _i, _i, _p],
     'di_branch_mix_f32': [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
+    'di_mha_small_rows_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _p, _i, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i,
+                                  _p],
+    'di_rows_scatter_add_f32': [_p, _i, _p, _p, _i, _i, _i, _p],
+    'di_branch_mix_bwd_f32': [_p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _p],
+    'di_pred_finish_pp_bwd_f32': [_p, _p, _p, _p, _i, _i, _i, _p],
     'di_rcnn_rois_f32': [_p, _i, _p, _p, _p, _p, _p, _i, _i, _i, _i, _fp, _p],
     'di_roi_align_f32': [_p, _p, _p, _i, _i, _i, _i, _f, _p],
     'di_dynconv_f32': [_p, _p, _p, _p, _p, _p, _p, _i, _f, _p],

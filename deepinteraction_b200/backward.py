@@ -456,9 +456,12 @@ def _rcnn_bw_pack(dec, bp):
     T = _transposed
     s = float(C // dec.num_heads) ** -0.5           # folded into the q rows of the packed in-projection (_pack_mha)
     qscale = torch.cat([torch.full((C,), s, dtype=torch.float64), torch.ones(2 * C, dtype=torch.float64)])
-    bp['_bw'] = dict(ffn1=T(bp['ffn'][0]), ffn2=T(bp['ffn'][2]), dout=T(bp['dout'][0]), dyn=bp['dyn'][0].w.t().contiguous(),
-                     attn_in=T(bp['attn'][0]), attn_out=T(bp['attn'][2]), qscale=fold.dev(qscale, bp['norm1'][0].device))
-    return bp['_bw']
+    bw = dict(ffn1=T(bp['ffn'][0]), ffn2=T(bp['ffn'][2]), dout=T(bp['dout'][0]), dyn=bp['dyn'][0].w.t().contiguous(),
+              attn_in=T(bp['attn'][0]), attn_out=T(bp['attn'][2]), qscale=fold.dev(qscale, bp['norm1'][0].device))
+    if bp['v2']:
+        bw.update(sffn1=T(bp['self_ffn'][0]), sffn2=T(bp['self_ffn'][2]))
+    bp['_bw'] = bw
+    return bw
 
 
 # the dX product of the DynamicConv generator: d q1 [B*P, C] = d params [B*P, 32768] W_dyn.  The tensor-core GEMM has no
@@ -467,14 +470,15 @@ def _rcnn_bw_pack(dec, bp):
 _DYN_SPLITS = 64
 
 
-def _v1_rcnn_block(dec, li, query, maps, image):
-    """-> (block pack, B, P) of decode_head[li], a V1 ImageRCNNBlock (image) or PointRCNNBlock (not image) read from maps
-    ([B*V, h, w, C] image maps or the [B, Y, X, C] BEV map); NotImplementedError before any launch for what the backward
-    of that block does not cover."""
-    fn, kind = ('image_rcnn_backward', 'ImageRCNNBlock') if image else ('point_rcnn_backward', 'PointRCNNBlock')
+def _rcnn_block_of(dec, li, query, maps, image, v2=False):
+    """-> (block pack, B, P) of decode_head[li], an ImageRCNNBlock[V2] (image) or PointRCNNBlock[V2] (not image) read from
+    maps ([B*V, h, w, C] image maps or the [B, Y, X, C] BEV map); NotImplementedError before any launch for what the
+    backward of that block does not cover."""
+    fn, kind = ('image_rcnn', 'ImageRCNNBlock') if image else ('point_rcnn', 'PointRCNNBlock')
+    fn, kind = (fn + '_v2_backward', kind + 'V2') if v2 else (fn + '_backward', 'V1 ' + kind)
     bp = dec.pack()['blocks'][li]
-    if bp['image'] != image or bp['v2']:
-        raise NotImplementedError('%s covers the V1 %s only (decode_head[%d] is %s)'
+    if bp['image'] != image or bp['v2'] != v2:
+        raise NotImplementedError('%s covers the %s only (decode_head[%d] is %s)'
                                   % (fn, kind, li, type(dec.decode_head[li]).__name__))
     C, M = dec.hidden_channel, query.shape[0]
     B = maps.shape[0] // dec.num_views if image else maps.shape[0]
@@ -501,6 +505,41 @@ def _rcnn_forward(dec, bp, query, pred, maps, img_metas, B, P, saved=None):
     return dec._rcnn_block(bp, query, pred, None, maps, B, P, prm, proj, aux, saved=saved)
 
 
+def _rcnn_middle_backward(dec, bp, bw, sv, maps, B, P, dq2, masks, R):
+    """The section of an RCNN block's backward that V1 and V2 blocks share, from d q2 down: norm2, DynamicConv (norm3 +
+    ReLU, out_layer, the dynamic convolution, the parameter generator), RoIAlign, norm1 and the self attention over the
+    queries of a sample (within the view groups of masks = (onbits, win) when given).  -> (dz1 [B*P, C]: the gradient
+    of norm1's input sum, whose residual part reaches the block's input; dqkv [B*P, 3C]: the gradient of the packed
+    in-projection's output; d_maps); the gradients of norm2, dyconv, norm1 and out_proj are stored in R."""
+    image = bp['image']
+    C, H = dec.hidden_channel, dec.num_heads
+    x = '' if image else '_pts'
+    dz2, R[f'norm2{x}.weight'], R[f'norm2{x}.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
+    D = f'dyconv{x}.'
+    dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
+    _put(R, (D + 'out_layer', _layer_grads(dzd3, sv['flat'])))
+    d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
+    dn = ops.col_sum(d_norm).view(4, C)
+    R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
+    _put(R, (D + 'dynamic_layer', _layer_grads(d_params, sv['q1'])))
+    dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
+    d_maps = ops.roi_align_bwd(d_roi, sv['rois'], *maps.shape[:3], 1.0 / dec.out_size_factor_img if image else 1.0)
+    dz1, R[f'norm1{x}.weight'], R[f'norm1{x}.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
+    dqkv, g_out = _self_attn_backward(dz1, sv['a'], sv['qkv'], bw['attn_out'], B, P, H, *masks)
+    _put(R, (f'dyconv_pre_self_attn{x}.out_proj', g_out))
+    return dz1, dqkv, d_maps
+
+
+def _in_proj_backward(bp, bw, query, dqkv, dz1, R):
+    """The block's input gradient d query = dqkv W_in + dz1 and the in-projection's gradients (into R)."""
+    A = 'dyconv_pre_self_attn%s.' % ('' if bp['image'] else '_pts')
+    d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
+    # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
+    dW_in, db_in = _layer_grads(dqkv, query)
+    R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = dW_in * bw['qscale'][:, None], db_in * bw['qscale']
+    return d_query
+
+
 def _v1_rcnn_backward(dec, bp, B, P, query, pred, maps, img_metas, grad_out):
     """Backward of a V1 RCNN block (reference models/utils/decoder_utils.py:632-761 image, :765-841 BEV), LayerNorms as
     they are, dropout off -> (d_query, d_maps, grads).  The block is re-run eagerly with its intermediates kept.  The two
@@ -508,7 +547,6 @@ def _v1_rcnn_backward(dec, bp, B, P, query, pred, maps, img_metas, grad_out):
     attention within a view group, rows on no live view written as 0) and the parameter names."""
     image = bp['image']
     query, pred, maps, grad_out = (t.contiguous() for t in (query, pred, maps, grad_out))
-    C, H = dec.hidden_channel, dec.num_heads
     sv = {}
     _rcnn_forward(dec, bp, query, pred, maps, img_metas, B, P, saved=sv)
     bw = _rcnn_bw_pack(dec, bp)
@@ -521,27 +559,50 @@ def _v1_rcnn_backward(dec, bp, B, P, query, pred, maps, img_metas, grad_out):
     dq2, n3, l2, l1 = _ffn_norm_backward(grad_out, sv['z3'], bp['norm3'][0], sv['f'], (ops.gelu_bwd, sv['h']), sv['q2'],
                                          bw['ffn2'], bw['ffn1'])
     _put(R, ('norm3' + x, n3), ('linear2' + x, l2), ('linear1' + x, l1))
-    # norm2, DynamicConv: norm3 + ReLU, out_layer, the dynamic convolution, the parameter generator, RoIAlign
-    dz2, R[f'norm2{x}.weight'], R[f'norm2{x}.bias'] = ops.ln_bwd(dq2, sv['z2'], bp['norm2'][0])
-    D = f'dyconv{x}.'
-    dzd3, R[D + 'norm3.weight'], R[D + 'norm3.bias'] = ops.ln_bwd(ops.relu_bwd(dz2, sv['t']), sv['zd3'], bp['dn3'][0])
-    _put(R, (D + 'out_layer', _layer_grads(dzd3, sv['flat'])))
-    d_roi, d_params, d_norm = ops.dynconv_bwd(sv['roi'], sv['params'], *bp['dn1'], *bp['dn2'], ops.linear([dzd3], bw['dout']))
-    dn = ops.col_sum(d_norm).view(4, C)
-    R[D + 'norm1.weight'], R[D + 'norm1.bias'], R[D + 'norm2.weight'], R[D + 'norm2.bias'] = dn.unbind(0)
-    _put(R, (D + 'dynamic_layer', _layer_grads(d_params, sv['q1'])))
-    dq1 = ops.rows_finish(ops.linear([d_params], bw['dyn'], splits=_DYN_SPLITS), res=dz2)
-    d_maps = ops.roi_align_bwd(d_roi, sv['rois'], *maps.shape[:3], 1.0 / dec.out_size_factor_img if image else 1.0)
-    # norm1, self attention over the queries of a sample (image blocks: within the view groups)
-    dz1, R[f'norm1{x}.weight'], R[f'norm1{x}.bias'] = ops.ln_bwd(dq1, sv['z1'], bp['norm1'][0])
-    A = f'dyconv_pre_self_attn{x}.'
-    dqkv, g_out = _self_attn_backward(dz1, sv['a'], sv['qkv'], bw['attn_out'], B, P, H, *masks)
-    _put(R, (A + 'out_proj', g_out))
-    d_query = ops.linear([dqkv], bw['attn_in'], res=dz1)
-    # dqkv is the gradient of the packed projection, whose q rows carry head_dim^-0.5
-    dW_in, db_in = _layer_grads(dqkv, query)
-    R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = dW_in * bw['qscale'][:, None], db_in * bw['qscale']
-    return d_query, d_maps, R
+    dz1, dqkv, d_maps = _rcnn_middle_backward(dec, bp, bw, sv, maps, B, P, dq2, masks, R)
+    return _in_proj_backward(bp, bw, query, dqkv, dz1, R), d_maps, R
+
+
+def _v2_rcnn_backward(dec, bp, B, P, query, pred, maps, img_metas, grad_out):
+    """Backward of a V2 RCNN block (reference models/utils/decoder_utils.py:844-991 image, :995-1089 BEV; oracle/mmpi_pp.py),
+    LayerNorms as they are, dropout off -> (d_query, d_maps, grads).  out = q3 * scale + s_l * self_scale, where q3 is
+    the V1 path up to q2 followed by norm3(q2 + ffn(q2)) (ReLU) and s_l = self_norm(q1_l + self_ffn(q1_l)) is the self
+    branch of the FIRST query of the row's (sample, view) group, q1_l = norm1(prev[lead] + out_proj(attention of the
+    leader over its group)).  The leader branch shares norm1, out_proj, the in-projection and the group's keys and values
+    with the main path, so its gradients are added to the main path's; a query that leads two views gets both."""
+    image = bp['image']
+    query, pred, maps, grad_out = (t.contiguous() for t in (query, pred, maps, grad_out))
+    C, H = dec.hidden_channel, dec.num_heads
+    sv = {}
+    _rcnn_forward(dec, bp, query, pred, maps, img_metas, B, P, saved=sv)
+    bw = _rcnn_bw_pack(dec, bp)
+    x = '' if image else '_pts'
+    Vg = dec.num_views if image else 1
+    R = {}
+    # the branch mix: image rows on no live view are written as 0 and take no gradient
+    dq3, d_s, R['scale'], R['self_scale'] = ops.branch_mix_bwd(grad_out, sv['q3'], sv['s_l'], sv['win'], bp['scale'],
+                                                               bp['self_scale'], P, Vg, image)
+    # main path: norm3, FFN (ReLU), then the section V1 blocks share
+    dq2, n3, l2, l1 = _ffn_norm_backward(dq3, sv['z3'], bp['norm3'][0], sv['f'], (ops.relu_bwd, sv['f']), sv['q2'],
+                                         bw['ffn2'], bw['ffn1'])
+    _put(R, ('norm3' + x, n3), ('ffn.layers.1', l2), ('ffn.layers.0.0', l1))
+    dz1, dqkv, d_maps = _rcnn_middle_backward(dec, bp, bw, sv, maps, B, P, dq2, (sv['onbits'], sv['win']) if image else (), R)
+    # leader branch on the B*Vg leader rows: self_norm, self FFN (ReLU), norm1, out_proj, the group attention
+    dq1_l, sn, s2, s1 = _ffn_norm_backward(d_s, sv['zs'], bp['self_norm'][0], sv['fs'], (ops.relu_bwd, sv['fs']), sv['q1_l'],
+                                           bw['sffn2'], bw['sffn1'])
+    _put(R, ('self_norm' + x, sn), ('self_ffn.layers.1', s2), ('self_ffn.layers.0.0', s1))
+    dz1_l, dg, db = ops.ln_bwd(dq1_l, sv['z1_l'], bp['norm1'][0])
+    R[f'norm1{x}.weight'], R[f'norm1{x}.bias'] = _add(R[f'norm1{x}.weight'], dg), _add(R[f'norm1{x}.bias'], db)
+    A = f'dyconv_pre_self_attn{x}.out_proj.'
+    dW, db = _layer_grads(dz1_l, sv['a_l'])
+    R[A + 'weight'], R[A + 'bias'] = _add(R[A + 'weight'], dW), _add(R[A + 'bias'], db)
+    da_l = ops.linear([dz1_l], bw['attn_out'])
+    qkv = sv['qkv']
+    dq_l = ops.mha_small_rows_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], da_l, B, P, H, sv['onbits'], sv['lrow'],
+                                  sv['lwin'], dqkv[:, C:2 * C], dqkv[:, 2 * C:])
+    ops.rows_scatter_add(dq_l, sv['lrow'], dqkv[:, :C])           # the leader's own query row
+    ops.rows_scatter_add(dz1_l, sv['lrow'], dz1)                  # norm1's residual: prev[lead]
+    return _in_proj_backward(bp, bw, query, dqkv, dz1, R), d_maps, R
 
 
 @_precise()
@@ -554,7 +615,7 @@ def point_rcnn_backward(dec, li, query, pred, bev, grad_out):
     dec.decode_head[li], keyed and shaped as in its state_dict).  The RoIs are constants (the reference computes them
     from detached predictions), so pred gets no gradient.  The block is re-run eagerly with its intermediates kept;
     everything stays on the device, without host synchronisation after the first call of a pack."""
-    bp, B, P = _v1_rcnn_block(dec, li, query, bev, False)
+    bp, B, P = _rcnn_block_of(dec, li, query, bev, False)
     d_query, d_bev, R = _v1_rcnn_backward(dec, bp, B, P, query, pred, bev, None, grad_out)
     return dict(d_query=d_query, d_bev=d_bev, grads=R)
 
@@ -572,7 +633,7 @@ def image_rcnn_backward(dec, li, query, pred, img, img_metas, grad_out):
     on no live view outputs the constant 0, so its grad_out row is ignored and its d_query row is 0.  The RoIs and view
     groups are constants (the reference computes them from detached predictions), so pred gets no gradient.  Everything
     stays on the device, without host synchronisation after the first call of a pack."""
-    bp, B, P = _v1_rcnn_block(dec, li, query, img, True)
+    bp, B, P = _rcnn_block_of(dec, li, query, img, True)
     d_query, d_img, R = _v1_rcnn_backward(dec, bp, B, P, query, pred, img, img_metas, grad_out)
     return dict(d_query=d_query, d_img=d_img, grads=R)
 
@@ -584,7 +645,7 @@ class PointRCNNFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, dec, li, query, pred, bev):
-        bp, B, P = _v1_rcnn_block(dec, li, query, bev, False)
+        bp, B, P = _rcnn_block_of(dec, li, query, bev, False)
         ctx.dec, ctx.li = dec, li
         ctx.save_for_backward(query, pred, bev)
         with _precise():
@@ -604,7 +665,7 @@ class ImageRCNNFunction(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, dec, li, query, pred, img, img_metas):
-        bp, B, P = _v1_rcnn_block(dec, li, query, img, True)
+        bp, B, P = _rcnn_block_of(dec, li, query, img, True)
         ctx.dec, ctx.li, ctx.img_metas = dec, li, img_metas
         ctx.save_for_backward(query, pred, img)
         with _precise():
@@ -617,7 +678,74 @@ class ImageRCNNFunction(torch.autograd.Function):
         return None, None, r['d_query'], None, r['d_img'], None
 
 
-# ---- decoder: prediction heads, heat-map head, query init and the whole base decoder from its loss ---------------------
+# ---- decoder: the V2 RCNN blocks of the ++ decoder, PointRCNNBlockV2 and ImageRCNNBlockV2 --------------------------------
+@_precise()
+def point_rcnn_v2_backward(dec, li, query, pred, bev, grad_out):
+    """Backward of the ++ decoder's PointRCNNBlockV2 (reference models/utils/decoder_utils.py:995-1089; dec.decode_head[li],
+    li = 1 or 3), LayerNorms as they are, dropout off.  Arguments as point_rcnn_backward's.  -> dict(d_query [B*P, C],
+    d_bev [B, Y, X, C], grads = {name: tensor} for the 32 parameters of dec.decode_head[li], keyed and shaped as in its
+    state_dict, scale and self_scale included).  One view group per sample: every row receives the self branch of the
+    sample's first query.  The RoIs are constants, so pred gets no gradient; no host synchronisation after the first call
+    of a pack."""
+    bp, B, P = _rcnn_block_of(dec, li, query, bev, False, v2=True)
+    d_query, d_bev, R = _v2_rcnn_backward(dec, bp, B, P, query, pred, bev, None, grad_out)
+    return dict(d_query=d_query, d_bev=d_bev, grads=R)
+
+
+@_precise()
+def image_rcnn_v2_backward(dec, li, query, pred, img, img_metas, grad_out):
+    """Backward of the ++ decoder's ImageRCNNBlockV2 (reference models/utils/decoder_utils.py:844-991; dec.decode_head[li],
+    li = 0 or 2), LayerNorms as they are, dropout off.  Arguments as image_rcnn_backward's.  -> dict(d_query [B*P, C],
+    d_img [B*V, h, w, C], grads = {name: tensor} for the 32 parameters of dec.decode_head[li]).  A query with win = w >= 0
+    receives the self branch of the first query on live view w of its sample; a query on no live view outputs 0, so its
+    grad_out row is ignored.  The RoIs and view groups are constants; no host synchronisation after the first call of a
+    pack."""
+    bp, B, P = _rcnn_block_of(dec, li, query, img, True, v2=True)
+    d_query, d_img, R = _v2_rcnn_backward(dec, bp, B, P, query, pred, img, img_metas, grad_out)
+    return dict(d_query=d_query, d_img=d_img, grads=R)
+
+
+class PointRCNNV2Function(torch.autograd.Function):
+    """autograd wrapper: out [B*P, C] = dec.decode_head[li] (a PointRCNNBlockV2) with the forward schedule's kernels, bit
+    for bit; backward -> (d_query, d_bev) through point_rcnn_v2_backward.  Parameter gradients are returned by
+    point_rcnn_v2_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, li, query, pred, bev):
+        bp, B, P = _rcnn_block_of(dec, li, query, bev, False, v2=True)
+        ctx.dec, ctx.li = dec, li
+        ctx.save_for_backward(query, pred, bev)
+        with _precise():
+            return _rcnn_forward(dec, bp, query.contiguous(), pred.contiguous(), bev.contiguous(), None, B, P)[0]
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        query, pred, bev = ctx.saved_tensors
+        r = point_rcnn_v2_backward(ctx.dec, ctx.li, query, pred, bev, grad_out)
+        return None, None, r['d_query'], None, r['d_bev']
+
+
+class ImageRCNNV2Function(torch.autograd.Function):
+    """autograd wrapper: out [B*P, C] = dec.decode_head[li] (an ImageRCNNBlockV2) with the forward schedule's kernels, bit
+    for bit; backward -> (d_query, d_img) through image_rcnn_v2_backward.  Parameter gradients are returned by
+    image_rcnn_v2_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, li, query, pred, img, img_metas):
+        bp, B, P = _rcnn_block_of(dec, li, query, img, True, v2=True)
+        ctx.dec, ctx.li, ctx.img_metas = dec, li, img_metas
+        ctx.save_for_backward(query, pred, img)
+        with _precise():
+            return _rcnn_forward(dec, bp, query.contiguous(), pred.contiguous(), img.contiguous(), img_metas, B, P)[0]
+
+    @staticmethod
+    def backward(ctx, grad_out):
+        query, pred, img = ctx.saved_tensors
+        r = image_rcnn_v2_backward(ctx.dec, ctx.li, query, pred, img, ctx.img_metas, grad_out)
+        return None, None, r['d_query'], None, r['d_img'], None
+
+
+# ---- decoder: prediction heads, heat-map head, query init and the whole decoder from its loss ---------------------
 def _pred_bw_pack(dec, li, pack):
     """Transposed weights of a prediction FFN's two dX products and, per head, its row / column ranges in the packed
     weights (mmpi._pack_pred) with the constants of fold.conv_bn_unfold, built once per pack.  li: index into
@@ -708,24 +836,29 @@ def heatmap_head_backward(dec, new_pts, grad_out):
     return dict(d_new_pts=dx, grads=R)
 
 
-def _decoder_checks(dec, pts_conv, new_pts, img):
-    """NotImplementedError before any launch for what decoder_backward does not cover, including what the block
-    backwards reject (_v1_rcnn_block): the maps' shapes and channels."""
+def _decoder_checks(dec, pts_conv, new_pts, img, plusplus=False):
+    """NotImplementedError before any launch for what decoder_backward (plusplus: decoder_pp_backward) does not cover,
+    including what the block backwards reject (_rcnn_block_of): the maps' shapes and channels."""
+    fn = 'decoder_pp_backward' if plusplus else 'decoder_backward'
     B, P, C = pts_conv.shape[0], dec.num_proposals, dec.hidden_channel
     bev = (B, dec.y_size, dec.x_size, C)
     if (pts_conv.dim() != 4 or tuple(pts_conv.shape) != bev or tuple(new_pts.shape) != bev or img.dim() != 4
             or img.shape[0] != B * dec.num_views or img.shape[3] != C or P > 512):
-        raise NotImplementedError(f'decoder_backward: pts_conv and new_pts must be [B, {dec.y_size}, {dec.x_size}, {C}] and '
+        raise NotImplementedError(f'{fn}: pts_conv and new_pts must be [B, {dec.y_size}, {dec.x_size}, {C}] and '
                                   f'img [B*{dec.num_views}, h, w, {C}], pixel-major (got {tuple(pts_conv.shape)}, '
                                   f'{tuple(new_pts.shape)}, {tuple(img.shape)})')
     from .mmpi import DeepInteractionPlusPlusDecoder
-    if isinstance(dec, DeepInteractionPlusPlusDecoder) or any(getattr(b, 'v2', False) for b in dec.decode_head):
+    v2 = [getattr(b, 'v2', False) for b in dec.decode_head]
+    if not plusplus and (isinstance(dec, DeepInteractionPlusPlusDecoder) or any(v2)):
         raise NotImplementedError('decoder_backward covers the base DeepInteractionDecoder only (the V2 RCNN blocks of the '
                                   '++ decoder have no backward)')
+    if plusplus and not (isinstance(dec, DeepInteractionPlusPlusDecoder) and all(v2)):
+        raise NotImplementedError('decoder_pp_backward covers the DeepInteractionPlusPlusDecoder only (the base decoder: '
+                                  'decoder_backward)')
     if not dec.auxiliary:
-        raise NotImplementedError('decoder_backward needs auxiliary=True (a loss on every layer), as both reference configs')
+        raise NotImplementedError(f'{fn} needs auxiliary=True (a loss on every layer), as both reference configs')
     if dec.num_heads != 8 or dec.hidden_channel != 128 or P > 256 or dec.num_classes_heat > 32 or B < 1:
-        raise NotImplementedError('decoder_backward: the gradient kernels take 8 heads x 16 channels, P <= 256 proposals '
+        raise NotImplementedError(f'{fn}: the gradient kernels take 8 heads x 16 channels, P <= 256 proposals '
                                   f'and K <= 32 classes (got heads={dec.num_heads}, C={dec.hidden_channel}, P={P}, '
                                   f'K={dec.num_classes_heat})')
 
@@ -733,6 +866,17 @@ def _decoder_checks(dec, pts_conv, new_pts, img):
 def _prefixed(R, prefix, grads):
     for k, v in grads.items():
         R[prefix + k] = v
+
+
+def _decoder_loss_forward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_labels_3d, grad_losses):
+    """The forward with the values the chain needs (the forward schedule's own kernels, run eagerly), the loss and its
+    gradient -> (saved values, forward result, losses, d dense heat-map logits, d prediction rows [L, B*P, NP])."""
+    proj, aux = (t.pin_memory().to(pts_conv.device, non_blocking=True) for t in dec._camera_consts(img_metas))
+    sv = {}
+    r = dec._schedule(pts_conv, new_pts, img, geom.input_hw(img_metas), proj, aux, sv)
+    losses = dec.loss(gt_bboxes_3d, gt_labels_3d, dec._outputs(r, pts_conv.shape[0]))
+    d_heat, d_pred = dec.loss_backward(grad_losses)
+    return sv, r, losses, d_heat, d_pred
 
 
 @_precise()
@@ -753,14 +897,9 @@ def decoder_backward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_la
     B, P = pts_conv.shape[0], dec.num_proposals
     _decoder_checks(dec, pts_conv, new_pts, img)
     pk = dec.pack()
-    dev_ = pts_conv.device
     pts_conv, new_pts, img = pts_conv.contiguous(), new_pts.contiguous(), img.contiguous()
-    # ---- forward with the values the chain needs: the forward schedule's own kernels, run eagerly
-    proj, aux = (t.pin_memory().to(dev_, non_blocking=True) for t in dec._camera_consts(img_metas))
-    sv = {}
-    r = dec._schedule(pts_conv, new_pts, img, geom.input_hw(img_metas), proj, aux, sv)
-    losses = dec.loss(gt_bboxes_3d, gt_labels_3d, dec._outputs(r, B))
-    d_heat, d_pred = dec.loss_backward(grad_losses)
+    sv, r, losses, d_heat, d_pred = _decoder_loss_forward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d,
+                                                          gt_labels_3d, grad_losses)
     # ---- MMPI layers in reverse: pred_head[l] reads [q_{l+1} | q_l]; block l maps q_l to q_{l+1} with the RoIs of the
     # previous layer's (detached) predictions
     qs = [sv['query_feat1']] + sv['layer_query']
@@ -789,10 +928,20 @@ def decoder_backward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_la
         dq = _add(d_q, ph['d_srcs'][1])
     # prediction_heads[0] reads the layer's output q1 and feeds the fallback rows (its RoIs are constants).  Under the
     # on-image mask those rows carry weight 0, so this is exactly zero in the base decoder; it is computed all the same.
-    pf = pred_head_backward(dec, None, [qs[0]], d_first if d_first is not None else torch.zeros_like(d_pred[0]))
+    d_first = d_first if d_first is not None else torch.zeros_like(d_pred[0])
+    d_pts_conv, d_new_pts, d_img = _decoder_tail(dec, sv, r, R, dq, d_first, d_heat, pts_conv, new_pts, img, d_new_pts, d_img)
+    return dict(losses=losses, d_pts_conv=d_pts_conv, d_new_pts=d_new_pts, d_img=d_img, grads=R)
+
+
+def _decoder_tail(dec, sv, r, R, dq, d_first, d_heat, pts_conv, new_pts, img, d_new_pts, d_img):
+    """The part of the decoder's gradient the base and the ++ decoder share, from d q1 (the transformer layer's output,
+    without prediction_heads[0]'s part) and d first (that head's output rows): prediction_heads[0], the transformer layer,
+    query init and the heat-map head.  -> (d_pts_conv, d_new_pts, d_img) with the MMPI layers' d_new_pts / d_img (None =
+    zero) added; parameter gradients are stored in R."""
+    B = pts_conv.shape[0]
+    pf = pred_head_backward(dec, None, [sv['query_feat1']], d_first)
     _prefixed(R, 'prediction_heads.0.', pf['grads'])
     dq = _add(dq, pf['d_srcs'][0])
-    # ---- transformer layer, query init, heat-map head
     rl = decoder_layer_backward(dec, sv['query_feat0'], sv['query_pos0'], pts_conv, dq)
     _prefixed(R, 'decoder.0.', rl['grads'])
     d_pts_conv = rl['d_bev'].contiguous()
@@ -804,7 +953,7 @@ def decoder_backward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_la
     d_new_pts = _add(d_new_pts, hh['d_new_pts'])
     if d_img is None:
         d_img = torch.zeros_like(img)
-    return dict(losses=losses, d_pts_conv=d_pts_conv, d_new_pts=d_new_pts, d_img=d_img, grads=R)
+    return d_pts_conv, d_new_pts, d_img
 
 
 class DecoderLossFunction(torch.autograd.Function):
@@ -826,4 +975,65 @@ class DecoderLossFunction(torch.autograd.Function):
         L = len(ctx.dec.decode_head)
         g = grad.reshape(1).float().expand(2 + 2 * L).contiguous()
         r = decoder_backward(ctx.dec, pts_conv, new_pts, img, *ctx.args, grad_losses=g)
+        return None, r['d_pts_conv'], r['d_new_pts'], r['d_img'], None, None, None
+
+
+@_precise()
+def decoder_pp_backward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_labels_3d, grad_losses=None):
+    """Gradient of the ++ decoder's losses (reference deepinteractionplusplus_decoder.py:200-319 forward, the base loss with
+    every layer's weights multiplied by that layer's on-image mask), BatchNorm in eval mode and dropout off.  Arguments
+    and result as decoder_backward's: dict(losses, d_pts_conv, d_new_pts, d_img, grads for every parameter but
+    heatmap_head.*).  Layer l's prediction rows are pred_head[l](q_{l+1}) with the look-forward centre (centre_l =
+    delta_l + look_l, look_{l+1} = delta_l + qpos_l, qpos and the first look detached), rows outside the cumulative mask
+    keep_l taking prediction_heads[0]'s rows at every layer (di_pred_finish_pp_bwd_f32 routes the gradient).  Those rows
+    carry weight 0 under the masks, so prediction_heads[0]'s gradient is exactly zero; it is computed all the same.
+    Proposals, RoIs, view groups, masks and the assignment are constants.  Everything stays on the device, without host
+    synchronisation after the first call of a pack."""
+    B, P = pts_conv.shape[0], dec.num_proposals
+    _decoder_checks(dec, pts_conv, new_pts, img, plusplus=True)
+    pk = dec.pack()
+    pts_conv, new_pts, img = pts_conv.contiguous(), new_pts.contiguous(), img.contiguous()
+    sv, r, losses, d_heat, d_pred = _decoder_loss_forward(dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d,
+                                                          gt_labels_3d, grad_losses)
+    d_delta, d_first = ops.pred_finish_pp_bwd(d_pred, torch.stack(r['keeps']))
+    # ---- MMPI layers in reverse: pred_head[l] reads q_{l+1}; block l maps q_l to q_{l+1} with the RoIs of the previous
+    # layer's (detached) predictions
+    qs = [sv['query_feat1']] + sv['layer_query']
+    R = {}
+    dq, d_img, d_new_pts = None, None, None
+    for li in reversed(range(len(pk['blocks']))):
+        bp = pk['blocks'][li]
+        ph = pred_head_backward(dec, li, [qs[li + 1]], d_delta[li])
+        _prefixed(R, 'pred_head.%d.' % li, ph['grads'])
+        pred_in = r['preds'][li - 1] if li > 0 else sv['first_res']
+        maps, metas = (img, img_metas) if bp['image'] else (new_pts, None)
+        dq, d_maps, g = _v2_rcnn_backward(dec, bp, B, P, qs[li], pred_in, maps, metas, _add(dq, ph['d_srcs'][0]))
+        if bp['image']:
+            d_img = _add(d_img, d_maps)
+        else:
+            d_new_pts = _add(d_new_pts, d_maps)
+        _prefixed(R, 'decode_head.%d.' % li, g)
+    d_pts_conv, d_new_pts, d_img = _decoder_tail(dec, sv, r, R, dq, d_first, d_heat, pts_conv, new_pts, img, d_new_pts, d_img)
+    return dict(losses=losses, d_pts_conv=d_pts_conv, d_new_pts=d_new_pts, d_img=d_img, grads=R)
+
+
+class DecoderPPLossFunction(torch.autograd.Function):
+    """autograd wrapper: the ++ decoder's summed loss from the encoder outputs pts_conv, new_pts [B, Y, X, C] and img
+    [B*V, h, w, C]; backward -> (d_pts_conv, d_new_pts, d_img) through decoder_pp_backward.  Parameter gradients are
+    returned by decoder_pp_backward."""
+
+    @staticmethod
+    def forward(ctx, dec, pts_conv, new_pts, img, img_metas, gt_bboxes_3d, gt_labels_3d):
+        _decoder_checks(dec, pts_conv, new_pts, img, plusplus=True)
+        ctx.dec, ctx.args = dec, (img_metas, gt_bboxes_3d, gt_labels_3d)
+        ctx.save_for_backward(pts_conv, new_pts, img)
+        losses = dec.loss(gt_bboxes_3d, gt_labels_3d, dec.forward_nhwc(pts_conv, new_pts, img, img_metas))
+        return torch.stack([v for k, v in losses.items() if 'loss' in k]).sum()
+
+    @staticmethod
+    def backward(ctx, grad):
+        pts_conv, new_pts, img = ctx.saved_tensors
+        L = len(ctx.dec.decode_head)
+        g = grad.reshape(1).float().expand(2 + 2 * L).contiguous()
+        r = decoder_pp_backward(ctx.dec, pts_conv, new_pts, img, *ctx.args, grad_losses=g)
         return None, r['d_pts_conv'], r['d_new_pts'], r['d_img'], None, None, None

@@ -362,23 +362,27 @@ mha_small_kernel(const float* __restrict__ q, int ldq, const float* __restrict__
 // tested here again (pass 1 leaves the invisible pairs of the workspace unwritten).  Neither pass reads the rows of a
 // masked pair.  Fixed summation orders (lanes over a strided index range, then the warp butterfly): deterministic, no
 // atomics; without a mask every pair is visible and the arithmetic is that of the unmasked form.
-template <int D>
+// ROWS: pass 1 of the row-map form (di_mha_small_rows_bwd_f32): warp (r, head) takes query rows[r] (-1: zero dq row) of
+// sample r / NI seen from group win[r]; dout and dq are indexed by r, and the workspace holds NI = rows_per_b columns.
+template <int D, bool ROWS>
 __global__ void __launch_bounds__(256)
 mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ k, int ldk, const float* __restrict__ v,
                        int ldv, const float* __restrict__ dout, int ldd, float* __restrict__ dq, int ldg, float* __restrict__ aw,
-                       float* __restrict__ sw, const int* __restrict__ onbits, const int* __restrict__ win, int B, int P, int Hh) {
+                       float* __restrict__ sw, const int* __restrict__ onbits, const int* __restrict__ win, int B, int P, int Hh,
+                       const int* __restrict__ rows, int NI) {
   const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
-  if (wid >= B * P * Hh) return;
-  const int head = wid % Hh, bq = wid / Hh, b = bq / P, i = bq % P;
-  const int wq = win ? win[bq] : 0;
+  if (wid >= B * NI * Hh) return;
+  const int head = wid % Hh, r = wid / Hh, b = r / NI, i = r % NI;
+  const int bq = ROWS ? rows[r] : r;
+  const int wq = ROWS ? (bq < 0 ? -1 : win[r]) : (win ? win[bq] : 0);
   if (wq < 0) {
-    if (lane < D) dq[(size_t)bq * ldg + head * D + lane] = 0.f;
+    if (lane < D) dq[(size_t)r * ldg + head * D + lane] = 0.f;
     return;
   }
   float qr[D], gr[D];
 #pragma unroll
   for (int d = 0; d < D; d += 4) {
-    const float4 a = ldg4(q + (size_t)bq * ldq + head * D + d), c = ldg4(dout + (size_t)bq * ldd + head * D + d);
+    const float4 a = ldg4(q + (size_t)bq * ldq + head * D + d), c = ldg4(dout + (size_t)r * ldd + head * D + d);
     qr[d] = a.x; qr[d + 1] = a.y; qr[d + 2] = a.z; qr[d + 3] = a.w;
     gr[d] = c.x; gr[d + 1] = c.y; gr[d + 2] = c.z; gr[d + 3] = c.w;
   }
@@ -427,14 +431,14 @@ mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __rest
   float acc[D];
 #pragma unroll
   for (int d = 0; d < D; ++d) acc[d] = 0.f;
-  const size_t col = ((size_t)(b * Hh + head) * P) * P + i;      // [b, head, j, i]
+  const size_t col = ((size_t)(b * Hh + head) * P) * NI + i;     // [b, head, j, i]
 #pragma unroll
   for (int n = 0; n < MAXK; ++n) {
     const int j = n * 32 + lane;
     if ((vis >> n) & 1) {
       const float ds = sc[n] * (dav[n] - dsum);
-      aw[col + (size_t)j * P] = sc[n];
-      sw[col + (size_t)j * P] = ds;
+      aw[col + (size_t)j * NI] = sc[n];
+      sw[col + (size_t)j * NI] = ds;
       const float* kr = k + (size_t)(b * P + j) * ldk + head * D;
 #pragma unroll
       for (int d = 0; d < D; d += 4) {
@@ -446,7 +450,7 @@ mha_small_bwd_q_kernel(const float* __restrict__ q, int ldq, const float* __rest
 #pragma unroll
   for (int d = 0; d < D; ++d) {
     const float a = warp_sum(acc[d]);
-    if (lane == d) dq[(size_t)bq * ldg + head * D + d] = a;
+    if (lane == d) dq[(size_t)r * ldg + head * D + d] = a;
   }
 }
 
@@ -488,6 +492,33 @@ mha_small_bwd_kv_kernel(const float* __restrict__ q, int ldq, const float* __res
       dv[(size_t)bj * ldg + head * D + d] = y;
     }
   }
+}
+
+// Pass 2 of the row-map form, one warp per (key j, head): lanes 0-15 hold dk_j's channels, lanes 16-31 dv_j's.  The warp
+// walks the NI leader rows of key j's sample in ascending r, skipping rows[r] = -1 and the rows whose group bit
+// rwin[r] key j lacks (as pass 1 does), and ADDS dk_j += sum_r dS_rj q_rows[r], dv_j += sum_r A_rj dO_r to the gradient
+// already there (the main attention's).
+template <int D>
+__global__ void __launch_bounds__(256)
+mha_small_rows_bwd_kv_kernel(const float* __restrict__ q, int ldq, const float* __restrict__ dout, int ldd,
+                             const float* __restrict__ aw, const float* __restrict__ sw, float* __restrict__ dk,
+                             float* __restrict__ dv, int ldg, const int* __restrict__ onbits, const int* __restrict__ rows,
+                             const int* __restrict__ rwin, int B, int P, int Hh, int NI) {
+  static_assert(2 * D == 32, "one lane per dk and per dv channel");
+  const int wid = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+  if (wid >= B * P * Hh) return;
+  const int head = wid % Hh, bj = wid / Hh, b = bj / P, j = bj % P;
+  const int bits = onbits[bj], d = lane & (D - 1);
+  const bool val = lane >= D;
+  const size_t col = ((size_t)(b * Hh + head) * P + j) * NI;
+  float acc = 0.f;
+  for (int i = 0; i < NI; ++i) {
+    const int r = b * NI + i, row = rows[r];
+    if (row < 0 || !((bits >> rwin[r]) & 1)) continue;
+    acc += val ? aw[col + i] * dout[(size_t)r * ldd + head * D + d] : sw[col + i] * q[(size_t)row * ldq + head * D + d];
+  }
+  float* g = (val ? dv : dk) + (size_t)bj * ldg + head * D + d;
+  *g += acc;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -944,6 +975,111 @@ __global__ void branch_mix_kernel(const float* __restrict__ a, const float* __re
     const float y = __fadd_rn(__fmul_rn(a[(size_t)m * C + c], s), __fmul_rn(l[c], t));
     out[(size_t)m * C + c] = (w < 0 && zero_off) ? 0.f : y;
   }
+}
+
+// dst[idx[r], :C] += src[r, :C] for r = 0..R-1 in order, rows with idx[r] < 0 skipped: one thread per column walks every
+// r, so equal indices are added in ascending r without atomics (R = B * V leader rows).
+__global__ void rows_scatter_add_kernel(const float* __restrict__ src, int lds, const int* __restrict__ idx, float* __restrict__ dst,
+                                        int ldd, int R, int C) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  for (int r = 0; r < R; ++r) {
+    const int i = idx[r];
+    if (i >= 0) dst[(size_t)i * ldd + c] += src[(size_t)r * lds + c];
+  }
+}
+
+// sum of v over a CTA of 128 threads in a fixed order (warp butterfly, then the 4 warps in order); valid in thread 0
+__device__ __forceinline__ float block128_sum(float v, float* red) {
+  v = warp_sum(v);
+  if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = v;
+  __syncthreads();
+  return ((red[0] + red[1]) + red[2]) + red[3];
+}
+
+// The (sample, view) group row m feeds in branch_mix_kernel: its win, or view 0 for win < 0 without zero_off; -1 when the
+// row is written as 0.
+__device__ __forceinline__ int branch_group(int w, int zero_off) { return w >= 0 ? w : (zero_off ? -1 : 0); }
+
+// Backward of branch_mix_kernel, one CTA of 128 per row m: da = dout * scale (0 on the zeroed rows) and the row's partial
+// sums of dout * a and dout * lead (the d scale and d self_scale terms) into part[2m], part[2m + 1].
+__global__ void __launch_bounds__(128)
+branch_mix_bwd_rows_kernel(const float* __restrict__ dout, const float* __restrict__ a, const float* __restrict__ lead,
+                           const int* __restrict__ win, const float* __restrict__ scale, float* __restrict__ da,
+                           float* __restrict__ part, int C, int P, int V, int zero_off) {
+  __shared__ float red[2][4];
+  const int m = blockIdx.x, g = branch_group(win[m], zero_off);
+  const float s = scale[0];
+  const float* l = lead + (size_t)((m / P) * V + (g < 0 ? 0 : g)) * C;
+  float ps = 0.f, pt = 0.f;
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    const float y = dout[(size_t)m * C + c];
+    da[(size_t)m * C + c] = g < 0 ? 0.f : y * s;
+    if (g >= 0) {
+      ps += y * a[(size_t)m * C + c];
+      pt += y * l[c];
+    }
+  }
+  ps = block128_sum(ps, red[0]);
+  pt = block128_sum(pt, red[1]);
+  if (threadIdx.x == 0) {
+    part[2 * m] = ps;
+    part[2 * m + 1] = pt;
+  }
+}
+
+// dlead[g = b * V + v] = self_scale * (sum of dout over the rows of sample b in group v, ascending row order): one CTA per
+// group, one thread per channel; 0 for a group no row belongs to.
+__global__ void branch_mix_bwd_lead_kernel(const float* __restrict__ dout, const int* __restrict__ win,
+                                           const float* __restrict__ self_scale, float* __restrict__ dlead, int C, int P,
+                                           int V, int zero_off) {
+  const int b = blockIdx.x / V, v = blockIdx.x % V;
+  const float t = self_scale[0];
+  for (int c = threadIdx.x; c < C; c += blockDim.x) {
+    float acc = 0.f;
+    for (int i = 0; i < P; ++i)
+      if (branch_group(win[b * P + i], zero_off) == v) acc += dout[(size_t)(b * P + i) * C + c];
+    dlead[(size_t)blockIdx.x * C + c] = t * acc;
+  }
+}
+
+// d scale = sum_m part[2m], d self_scale = sum_m part[2m + 1]: one CTA of 128, each thread over m = t, t + 128, ...
+__global__ void __launch_bounds__(128)
+branch_mix_bwd_scales_kernel(const float* __restrict__ part, float* __restrict__ d_scale, float* __restrict__ d_self_scale,
+                             int M) {
+  __shared__ float red[2][4];
+  float ps = 0.f, pt = 0.f;
+  for (int m = threadIdx.x; m < M; m += blockDim.x) {
+    ps += part[2 * m];
+    pt += part[2 * m + 1];
+  }
+  ps = block128_sum(ps, red[0]);
+  pt = block128_sum(pt, red[1]);
+  if (threadIdx.x == 0) {
+    d_scale[0] = ps;
+    d_self_scale[0] = pt;
+  }
+}
+
+// Backward of the ++ prediction finish over all L layers, one thread per (row m, column c): pred_l = keep_l ? delta_l (+ look_l
+// on the centre) : first, look_{l+1} = delta_l[:, 0:2] + qpos_l (qpos and the first look detached), so
+// d delta_l = keep_l dpred_l (+ keep_{l+1} dpred_{l+1} on columns 0, 1) and d first = sum_l !keep_l dpred_l, l ascending.
+__global__ void pred_finish_pp_bwd_kernel(const float* __restrict__ dpred, const int* __restrict__ keep,
+                                          float* __restrict__ d_delta, float* __restrict__ d_first, int L, int M, int NP) {
+  const int e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= M * NP) return;
+  const int m = e / NP, c = e % NP;
+  const size_t LS = (size_t)M * NP;
+  float f = 0.f;
+  for (int l = 0; l < L; ++l) {
+    const float g = dpred[l * LS + e];
+    const bool k = keep[(size_t)l * M + m] != 0;
+    float d = k ? g : 0.f;
+    if (c < 2 && l + 1 < L && keep[(size_t)(l + 1) * M + m]) d += dpred[(l + 1) * LS + e];
+    d_delta[l * LS + e] = d;
+    if (!k) f += g;
+  }
+  d_first[e] = f;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -1833,8 +1969,8 @@ int di_mha_small_bwd_f32(const float* q, int ldq, const float* k, int ldk, const
   const int warps = B * P * heads;
   float* aw = work;
   float* sw = work + (size_t)B * heads * P * P;
-  mha_small_bwd_q_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, ldg, aw, sw, onbits,
-                                                                    win, B, P, heads);
+  mha_small_bwd_q_kernel<16, false><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, ldg, aw, sw,
+                                                                           onbits, win, B, P, heads, nullptr, P);
   DI_CHECK_LAUNCH("di_mha_small_bwd_f32");
   mha_small_bwd_kv_kernel<16><<<di_cdiv(warps, 8), 256, 0, stream>>>(q, ldq, dout, ldd, aw, sw, dk, dv, ldg, onbits, win, B, P,
                                                                      heads);
@@ -1893,6 +2029,61 @@ int di_pred_finish_pp_f32(float* pred, float* qpos, float* look, const float* fi
                "di_pred_finish_pp_f32: bad argument");
   pred_finish_pp_kernel<<<di_cdiv(M, 128), 128, 0, stream>>>(pred, qpos, look, first, win, keep, first_layer, M, NP);
   DI_CHECK_LAUNCH("di_pred_finish_pp_f32");
+  return DI_OK;
+}
+
+// Backward of di_mha_small_rows_f32: dout [R, ldd] -> dq [R, lddq] (rows[r] = -1: zero row); dk / dv [B*P, ldg] are ADDED
+// to.  work: float [2 * B * heads * P * rows_per_b].
+int di_mha_small_rows_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout,
+                              int ldd, float* dq, int lddq, float* dk, float* dv, int ldg, float* work, const int* onbits,
+                              const int* rows, const int* rwin, int R, int rows_per_b, int B, int P, int heads, int head_dim,
+                              cudaStream_t stream) {
+  DI_CHECK_ARG(q && k && v && dout && dq && dk && dv && work && onbits && rows && rwin && B > 0 && rows_per_b > 0 &&
+               R == B * rows_per_b && P > 0 && P <= 512 && heads > 0 && head_dim == 16,
+               "di_mha_small_rows_bwd_f32: unsupported shape (head_dim=%d P=%d R=%d)", head_dim, P, R);
+  DI_CHECK_ARG(ldq % 4 == 0 && ldk % 4 == 0 && ldv % 4 == 0 && ldd % 4 == 0, "di_mha_small_rows_bwd_f32: strides must be multiples of 4");
+  float* aw = work;
+  float* sw = work + (size_t)B * heads * P * rows_per_b;
+  mha_small_bwd_q_kernel<16, true><<<di_cdiv(R * heads, 8), 256, 0, stream>>>(q, ldq, k, ldk, v, ldv, dout, ldd, dq, lddq, aw,
+                                                                              sw, onbits, rwin, B, P, heads, rows, rows_per_b);
+  DI_CHECK_LAUNCH("di_mha_small_rows_bwd_f32");
+  mha_small_rows_bwd_kv_kernel<16><<<di_cdiv(B * P * heads, 8), 256, 0, stream>>>(q, ldq, dout, ldd, aw, sw, dk, dv, ldg, onbits,
+                                                                                 rows, rwin, B, P, heads, rows_per_b);
+  DI_CHECK_LAUNCH("di_mha_small_rows_bwd_f32 (keys)");
+  return DI_OK;
+}
+
+// dst[idx[r], :C] += src[r, :C], r ascending, idx[r] < 0 skipped (the adjoint of di_take_rows_f32)
+int di_rows_scatter_add_f32(const float* src, int lds, const int* idx, float* dst, int ldd, int R, int C, cudaStream_t stream) {
+  DI_CHECK_ARG(src && idx && dst && R > 0 && C > 0, "di_rows_scatter_add_f32: bad argument");
+  rows_scatter_add_kernel<<<di_cdiv(C, 128), 128, 0, stream>>>(src, lds, idx, dst, ldd, R, C);
+  DI_CHECK_LAUNCH("di_rows_scatter_add_f32");
+  return DI_OK;
+}
+
+// Backward of di_branch_mix_f32: dout [M, C] -> da [M, C], dlead [M / P * V, C], d_scale [1], d_self_scale [1].
+// work: float [2 * M].
+int di_branch_mix_bwd_f32(const float* dout, const float* a, const float* lead, const int* win, const float* scale,
+                          const float* self_scale, float* da, float* dlead, float* d_scale, float* d_self_scale, float* work,
+                          int M, int C, int P, int V, int zero_off, cudaStream_t stream) {
+  DI_CHECK_ARG(dout && a && lead && win && scale && self_scale && da && dlead && d_scale && d_self_scale && work && M > 0 &&
+               C > 0 && P > 0 && V > 0 && M % P == 0, "di_branch_mix_bwd_f32: bad argument");
+  branch_mix_bwd_rows_kernel<<<M, 128, 0, stream>>>(dout, a, lead, win, scale, da, work, C, P, V, zero_off);
+  DI_CHECK_LAUNCH("di_branch_mix_bwd_f32");
+  branch_mix_bwd_lead_kernel<<<M / P * V, 128, 0, stream>>>(dout, win, self_scale, dlead, C, P, V, zero_off);
+  DI_CHECK_LAUNCH("di_branch_mix_bwd_f32 (leaders)");
+  branch_mix_bwd_scales_kernel<<<1, 128, 0, stream>>>(work, d_scale, d_self_scale, M);
+  DI_CHECK_LAUNCH("di_branch_mix_bwd_f32 (scales)");
+  return DI_OK;
+}
+
+// Backward of di_pred_finish_pp_f32 over the L layers: dpred [L, M, NP], keep [L, M] (each layer's cumulative mask) ->
+// d_delta [L, M, NP] (the gradient of each prediction head's output rows), d_first [M, NP].
+int di_pred_finish_pp_bwd_f32(const float* dpred, const int* keep, float* d_delta, float* d_first, int L, int M, int NP,
+                              cudaStream_t stream) {
+  DI_CHECK_ARG(dpred && keep && d_delta && d_first && L > 0 && M > 0 && NP >= 2, "di_pred_finish_pp_bwd_f32: bad argument");
+  pred_finish_pp_bwd_kernel<<<di_cdiv(M * NP, 128), 128, 0, stream>>>(dpred, keep, d_delta, d_first, L, M, NP);
+  DI_CHECK_LAUNCH("di_pred_finish_pp_bwd_f32");
   return DI_OK;
 }
 

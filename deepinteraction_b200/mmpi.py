@@ -535,8 +535,8 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         """One RCNN block of the MMPI layers (decoder_utils.py:632-1089) on query rows: prev [B*P, C], pred [B*P, NP] (the
         previous layer's predictions, which give the RoIs), new_pts [B, Y, X, C] (BEV blocks) or img [B*V, h, w, C] (image
         blocks) -> (rows [B*P, C], rois [B*P, 5], win [B*P]).  The one implementation of the block, for the forward
-        schedule and for the eager re-run of backward.point_rcnn_backward and backward.image_rcnn_backward; saved (a dict,
-        V1 blocks) additionally stores the values the backward needs, with the returned rows unchanged."""
+        schedule and for the eager re-run of the block backwards in backward.py; saved (a dict) additionally stores the
+        values the backward needs, with the returned rows unchanged."""
         C, H, V = self.hidden_channel, self.num_heads, self.num_views
         if bp['image']:
             rois, win, onbits = ops.rcnn_rois(pred, B, P, V, 0, prm, proj, aux)
@@ -556,6 +556,11 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
         t = ops.rows_finish(part, bias=bp['dout'][1], gamma=bp['dn3'][0], beta=bp['dn3'][1], act=ops.ACT_RELU)
         q2 = ops.rows_finish(t, res=q1, gamma=bp['norm2'][0], beta=bp['norm2'][1])
         f1w, f1b, f2w, f2b = bp['ffn']
+        if saved is not None:
+            # pre-norm sums and the hidden rows of the two-layer MLPs, which the fused row kernels do not return
+            saved.update(rois=rois, win=win, onbits=onbits, qkv=qkv, a=a, z1=self._mlp([a], wo, bo, res=prev), q1=q1, params=params, roi=roi,
+                         flat=flat, part=part, zd3=ops.rows_finish(part, bias=bp['dout'][1]), t=t,
+                         z2=ops.rows_finish(t, res=q1), q2=q2)
         if bp['v2']:
             # decoder_utils.py:971-988 / :1071-1085.  The self branch every query of a (sample, view) group receives
             # is the one of the group's FIRST query (the reference's (1,n,C) + (n,1,C) broadcast followed by [0];
@@ -567,16 +572,19 @@ class DeepInteractionDecoder(nn.Module, LossMixin):
             q1_l = self._mlp([a_l], wo, bo, res=ops.take_rows(prev, lrow), ln=bp['norm1'])
             s1w, s1b, s2w, s2b = bp['self_ffn']
             s_l = self._mlp([q1_l], s1w, s1b, ops.ACT_RELU, s2w, s2b, res=q1_l, ln=bp['self_norm'])
+            if saved is not None:
+                f = self._mlp([q2], f1w, f1b, ops.ACT_RELU)
+                fs = self._mlp([q1_l], s1w, s1b, ops.ACT_RELU)
+                saved.update(f=f, z3=self._mlp([f], f2w, f2b, res=q2), q3=q3, lrow=lrow, lwin=lwin, a_l=a_l,
+                             z1_l=self._mlp([a_l], wo, bo, res=ops.take_rows(prev, lrow)), q1_l=q1_l, fs=fs,
+                             zs=self._mlp([fs], s2w, s2b, res=q1_l), s_l=s_l)
             return ops.branch_mix(q3, s_l, win, bp['scale'], bp['self_scale'], P, Vg, bp['image']), rois, win
         q = self._mlp([q2], f1w, f1b, ops.ACT_GELU, f2w, f2b, res=q2, ln=bp['norm3'],
                       zero_if_neg=win if bp['image'] else None)
         if saved is not None:
-            # pre-norm sums and the FFN's hidden rows, which the fused row kernels do not return
             h = self._mlp([q2], f1w, f1b)
             f = self._mlp([q2], f1w, f1b, ops.ACT_GELU)
-            saved.update(rois=rois, win=win, onbits=onbits, qkv=qkv, a=a, z1=self._mlp([a], wo, bo, res=prev), q1=q1, params=params, roi=roi,
-                         flat=flat, part=part, zd3=ops.rows_finish(part, bias=bp['dout'][1]), t=t,
-                         z2=ops.rows_finish(t, res=q1), q2=q2, h=h, f=f, z3=self._mlp([f], f2w, f2b, res=q2))
+            saved.update(h=h, f=f, z3=self._mlp([f], f2w, f2b, res=q2))
         return q, rois, win
 
     def _to_dict(self, pred, B, P):

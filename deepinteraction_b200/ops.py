@@ -604,6 +604,50 @@ def branch_mix(a, lead, win, scale, self_scale, P, V, zero_off):
     return out
 
 
+def branch_mix_bwd(dout, a, lead, win, scale, self_scale, P, V, zero_off):
+    """Gradient of branch_mix: dout [M, C] -> (da [M, C], dlead [M / P * V, C], d scale [1], d self_scale [1])."""
+    M, C = a.shape
+    assert dout.is_contiguous() and a.is_contiguous() and lead.is_contiguous() and lead.shape == (M // P * V, C)
+    dev_ = a.device
+    da, dlead = torch.empty(M, C, device=dev_), torch.empty(M // P * V, C, device=dev_)
+    ds, dt, work = torch.empty(1, device=dev_), torch.empty(1, device=dev_), torch.empty(2 * M, device=dev_)
+    _call('di_branch_mix_bwd_f32', _ptr(dout), _ptr(a), _ptr(lead), _ptr(win), _ptr(scale), _ptr(self_scale), _ptr(da),
+          _ptr(dlead), _ptr(ds), _ptr(dt), _ptr(work), M, C, P, V, 1 if zero_off else 0, _stream(), launches=3)
+    return da, dlead, ds, dt
+
+
+def mha_small_rows_bwd(q, k, v, dout, B, P, heads, onbits, rows, rwin, dk, dv):
+    """Gradient of mha_small_rows: dout [R, C] -> dq [R, C] (rows[r] = -1: zero row); the key and value gradients are
+    ADDED to the rows of dk / dv [B*P, C] (views with one leading dimension, e.g. columns of mha_small_bwd's dqkv)."""
+    C, R = q.shape[1], rows.shape[0]
+    dq = torch.empty(R, C, device=q.device, dtype=torch.float32)
+    work = torch.empty(2 * B * heads * P * (R // B), device=q.device, dtype=torch.float32)
+    (pq, lq), (pk, lk), (pv, lv), (pd, ld), (pgk, lg), (pgv, lgv) = (_rows(t) for t in (q, k, v, dout, dk, dv))
+    assert lg == lgv and dk.shape == dv.shape == (B * P, C)
+    _call('di_mha_small_rows_bwd_f32', pq, lq, pk, lk, pv, lv, pd, ld, _ptr(dq), C, pgk, pgv, lg, _ptr(work), _ptr(onbits),
+          _ptr(rows), _ptr(rwin), R, R // B, B, P, heads, C // heads, _stream(), launches=2)
+    return dq
+
+
+def rows_scatter_add(src, idx, dst):
+    """dst[idx[r]] += src[r] in place (r ascending; idx[r] = -1 skipped): the adjoint of take_rows.  dst: rows view."""
+    R, C = src.shape
+    (ps, ls), (pd, ld) = _rows(src), _rows(dst)
+    assert dst.shape[1] == C and idx.shape[0] == R
+    _call('di_rows_scatter_add_f32', ps, ls, _ptr(idx), pd, ld, R, C, _stream())
+    return dst
+
+
+def pred_finish_pp_bwd(dpred, keep):
+    """Gradient of the L layers' pred_finish_pp: dpred [L, M, NP], keep [L, M] int32 (each layer's mask) -> (d_delta
+    [L, M, NP], the gradient of each prediction head's output rows; d_first [M, NP])."""
+    L, M, NP = dpred.shape
+    assert dpred.is_contiguous() and keep.is_contiguous() and keep.shape == (L, M) and keep.dtype == torch.int32
+    d_delta, d_first = torch.empty_like(dpred), torch.empty(M, NP, device=dpred.device)
+    _call('di_pred_finish_pp_bwd_f32', _ptr(dpred), _ptr(keep), _ptr(d_delta), _ptr(d_first), L, M, NP, _stream())
+    return d_delta, d_first
+
+
 def rcnn_rois(pred, B, P, V, mode, params10, proj=None, aux=None):
     dev = pred.device
     rois = torch.empty(B * P, 5, device=dev, dtype=torch.float32)

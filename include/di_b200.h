@@ -287,6 +287,23 @@ int di_mha_small_rows_f32(const float* q, int ldq, const float* k, int ldk, cons
 int di_take_rows_f32(const float* src, int ld, const int* idx, float* out, int R, int C, cudaStream_t stream);
 int di_branch_mix_f32(const float* a, const float* lead, const int* win, const float* scale, const float* self_scale,
                       float* out, int M, int C, int P, int V, int zero_off, cudaStream_t stream);
+/* their backward.  di_mha_small_rows_bwd_f32: dout [R, ldd] -> dq [R, lddq] (rows[r] = -1: zero row), the key and value
+ * gradients ADDED to dk / dv [B*P, ldg] (after di_mha_small_bwd_f32 has written the main attention's); work: float
+ * [2 * B * heads * P * rows_per_b].  di_rows_scatter_add_f32: dst[idx[r]] += src[r], r ascending, idx[r] = -1 skipped (the
+ * adjoint of di_take_rows_f32).  di_branch_mix_bwd_f32: da = scale * dout (0 on zeroed rows), dlead [M / P * V, C] =
+ * self_scale * the sum of dout over each group's rows, d_scale / d_self_scale [1] in fixed-order two-level sums; work:
+ * float [2 * M].  di_pred_finish_pp_bwd_f32: dpred [L, M, NP] and the per-layer keep [L, M] of di_pred_finish_pp_f32 ->
+ * d_delta [L, M, NP] (each prediction head's output gradient), d_first [M, NP].  Deterministic, no atomics. */
+int di_mha_small_rows_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* dout,
+                              int ldd, float* dq, int lddq, float* dk, float* dv, int ldg, float* work, const int* onbits,
+                              const int* rows, const int* rwin, int R, int rows_per_b, int B, int P, int heads, int head_dim,
+                              cudaStream_t stream);
+int di_rows_scatter_add_f32(const float* src, int lds, const int* idx, float* dst, int ldd, int R, int C, cudaStream_t stream);
+int di_branch_mix_bwd_f32(const float* dout, const float* a, const float* lead, const int* win, const float* scale,
+                          const float* self_scale, float* da, float* dlead, float* d_scale, float* d_self_scale, float* work,
+                          int M, int C, int P, int V, int zero_off, cudaStream_t stream);
+int di_pred_finish_pp_bwd_f32(const float* dpred, const int* keep, float* d_delta, float* d_first, int L, int M, int NP,
+                              cudaStream_t stream);
 /* box decode + RoI rectangles: image mode 0 (models/utils/decoder_utils.py:660-741), BEV mode 1 (:788-819);
  * core/bbox/coders/transfusion_bbox_coder.py:59-76 */
 int di_rcnn_rois_f32(const float* pred, int NP, const float* proj, const float* aux, float* rois, int* win, int* onbits,

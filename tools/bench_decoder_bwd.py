@@ -1,6 +1,6 @@
 """Time the gradient of the base decoder's losses on one GPU, next to the byte floors of its two new kernels.
 
-    python tools/bench_decoder_bwd.py [--batches 1 2] [--iters 20] [--warmup 5] [--floors-only]
+    python tools/bench_decoder_bwd.py [--batches 1 2] [--iters 20] [--warmup 5] [--floors-only] [--plusplus]
 
 At the base shapes (P = 200 proposals, C = 128, 180 x 180 BEV maps, 6 x 112 x 200 image maps of a 6-camera rig, K = 10
 classes, 4 MMPI layers) and per batch size, CUDA events time
@@ -9,7 +9,9 @@ classes, 4 MMPI layers) and per batch size, CUDA events time
   * backward.pred_head_backward of pred_head[0] (input [q | prev], 2C),
   * backward.heatmap_head_backward (two 3x3 convolutions on the 180 x 180 map),
   * the whole backward.decoder_backward (eager forward, loss, loss gradient and every block backward).
-The two kernels are printed with their byte floor at the data-sheet HBM bandwidth of the H100 SXM (3.35 TB/s).  The GPU
+With --plusplus the ++ decoder (V2 RCNN blocks) at the same shapes is timed instead: di_pred_finish_pp_bwd_f32 (the
+look-forward centre and fallback gradient), backward.pred_head_backward of pred_head[0] (input q, C) and the whole
+backward.decoder_pp_backward.  The two kernels are printed with their byte floor at the data-sheet HBM bandwidth of the H100 SXM (3.35 TB/s).  The GPU
 name, power limit and maximum SM clock come from nvidia-smi in the same run.  There is no CPU path: without a GPU the
 script fails (after printing the floors with --floors-only).
 """
@@ -38,12 +40,12 @@ def floors(B):
     return out
 
 
-def train_decoder():
-    """The base-shape decoder of tools/bench_decoder_layer_bwd.py with the reference's training configuration (Hungarian
-    assignment, L1 loss weight 0.25)."""
+def train_decoder(plusplus=False):
+    """The base-shape decoder (plusplus: the ++ decoder) of tools/bench_decoder_layer_bwd.py with the reference's training
+    configuration (Hungarian assignment, L1 loss weight 0.25)."""
     from deepinteraction_b200 import loss as Lm
     from tools import make_goldens as mg
-    m = _decoder()
+    m = _decoder(plusplus)
     tc = dict(mg.DEC_TRAIN_CFG, grid_size=[1440, 1440, 40], voxel_size=[0.075, 0.075, 0.2])
     m.train_cfg = tc
     m.bbox_assigner = Lm._build(Lm.ASSIGNERS, tc['assigner'])
@@ -70,12 +72,28 @@ def frame(m, B, g, d):
     return pts, new_pts, img, metas, gts, gls
 
 
+def plusplus_times(m, args, B, d):
+    """{name: callable} of the ++ decoder's backward pieces at batch B."""
+    import torch
+    from deepinteraction_b200 import backward, ops
+    backward.decoder_pp_backward(m, *args)                    # builds the per-pack tensors; leaves the loss targets
+    _, d_pred = m.loss_backward()
+    keep = torch.randint(0, 2, (L, B * P), device=d, dtype=torch.int32)
+    q = torch.randn(B * P, C, device=d)
+    return {
+        'di_pred_finish_pp_bwd_f32': lambda: ops.pred_finish_pp_bwd(d_pred, keep),
+        'pred_head_backward[0]': lambda: backward.pred_head_backward(m, 0, [q], d_pred[0]),
+        'decoder_pp_backward': lambda: backward.decoder_pp_backward(m, *args),
+    }
+
+
 def main(argv=None):
     ap = argparse.ArgumentParser(description=__doc__.split('\n')[0])
     ap.add_argument('--batches', type=int, nargs='+', default=[1, 2])
     ap.add_argument('--iters', type=int, default=20)
     ap.add_argument('--warmup', type=int, default=5)
     ap.add_argument('--floors-only', action='store_true')
+    ap.add_argument('--plusplus', action='store_true', help='time the ++ decoder\'s backward (decoder_pp_backward)')
     a = ap.parse_args(argv)
     for B in a.batches:
         for name, (nb, us) in floors(B).items():
@@ -88,11 +106,17 @@ def main(argv=None):
         raise SystemExit('no GPU: nothing is timed')
     d = torch.device('cuda:0')
     print(json.dumps(dict(gpu=gpu_info())))
-    m = train_decoder()
+    m = train_decoder(a.plusplus)
     for B in a.batches:
         g = torch.Generator().manual_seed(B)
         args = frame(m, B, g, d)
         pts, new_pts, img, metas, gts, gls = args
+        if a.plusplus:
+            times = plusplus_times(m, args, B, d)
+            for name, fn in times.items():
+                med, best = _time(fn, a.iters, a.warmup)
+                print(json.dumps(dict(B=B, what=name, median_us=round(med, 1), min_us=round(best, 1))))
+            continue
         r = backward.decoder_backward(m, *args)                 # builds the per-pack tensors; leaves the loss targets
         d_heat, d_pred = m.loss_backward()
         sv = {}

@@ -65,7 +65,7 @@ def _time(fn, iters, warmup):
     return times[len(times) // 2], times[0]
 
 
-def _decoder():
+def _decoder(plusplus=False):
     import torch
     from deepinteraction_b200 import mmpi, synth
     test_cfg = dict(dataset='nuScenes', grid_size=[1440, 1440, 40], out_size_factor=8, pc_range=[-54.0, -54.0],
@@ -73,7 +73,8 @@ def _decoder():
     coder = dict(type='TransFusionBBoxCoder', pc_range=[-54.0, -54.0], voxel_size=[0.075, 0.075], out_size_factor=8,
                  post_center_range=[-61.2, -61.2, -10.0, 61.2, 61.2, 10.0], score_threshold=0.0, code_size=10)
     torch.manual_seed(0)
-    m = mmpi.DeepInteractionDecoder(num_views=6, num_proposals=P, hidden_channel=C, num_classes=10, num_heads=HEADS,
+    cls = mmpi.DeepInteractionPlusPlusDecoder if plusplus else mmpi.DeepInteractionDecoder
+    m = cls(num_views=6, num_proposals=P, hidden_channel=C, num_classes=10, num_heads=HEADS,
                                     initialize_by_heatmap=True, nms_kernel_size=3, ffn_channel=256,
                                     common_heads=dict(center=(2, 2), height=(1, 2), dim=(3, 2), rot=(2, 2), vel=(2, 2)),
                                     loss_cls=dict(type='FocalLoss', use_sigmoid=True, gamma=2, alpha=0.25, reduction='mean'),
