@@ -7,7 +7,6 @@ import sys
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
 
 from conftest import rel_err
 from golden_sample import golden_err
@@ -45,19 +44,10 @@ def test_msdeform_kernel_matches_oracle_core(L):
 
 
 def test_seq_attn_matches_softmax_attention():
-    from deepinteraction_b200 import ops
-    g = torch.Generator().manual_seed(9)
-    G_, Wn, Lq, Lk, H, d = 3, 7, 60, 28, 8, 16
-    C = H * d
-    q = torch.randn(G_, Lq, Wn, C, generator=g)
-    k = torch.randn(G_, Lk, Wn, C, generator=g)
-    v = torch.randn(G_, Lk, Wn, C, generator=g)
-    sp = lambda t: t.permute(0, 2, 1, 3).reshape(G_ * Wn, -1, H, d).transpose(1, 2)      # (seq, H, L, d)
-    want = F.scaled_dot_product_attention(sp(q), sp(k), sp(v))                             # scale 1/sqrt(16)
-    want = want.transpose(1, 2).reshape(G_, Wn, Lq, C).permute(0, 2, 1, 3)
-    rows = lambda t: t.reshape(-1, C).contiguous().to(dev())
-    got = ops.seq_attn(rows(q), rows(k), rows(v), G_, Wn, Lq, Lk, H).view(G_, Lq, Wn, C).cpu()
-    assert rel_err(got, want) < 1e-5
+    """di_seq_attn_f32 at G = 3, Wn = 7, Lq = 60, Lk = 28, 8 heads, through the float64 per-head check that
+    test_gpu_polar_kernels.py runs over every other shape."""
+    from test_gpu_polar_kernels import check_seq_attn
+    check_seq_attn((3, 7, 60, 28, 8, False))
 
 
 def _build_pair(polar, seed):
