@@ -67,6 +67,12 @@ SIGNATURES = {
     'di_seq_attn_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p],
     'di_polar_gather_f32': [_p, _p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _f, _f, _p],
     'di_scatter_rows_add_f32': [_p, _p, _p, _p, _i, _i, _i, _i, _p, _p],
+    'di_msdeform_bwd_f32': [_p, _p, _p, _i, _p, _i, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i,
+                            ctypes.POINTER(ctypes.c_int), _p],
+    'di_seq_attn_bwd_f32': [_p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _p, _i, _i, _i, _i, _i, _i, _i, _p],
+    'di_polar_gather_bwd_f32': [_p, _p, _p, _p, _p, _i, _i, _i, _i, _i, _i, _i, _i, _i, _fp, _f, _f, _p],
+    'di_axpy_bwd_workspace': [],
+    'di_axpy_bwd_f32': [_p, _p, _p, _p, _p, _p, _ll, _p],
     # decoder.cu
     'di_heatmap_nms_f32': [_p, _p, _i, _p, _p, _i, _i, _i, _i, _i, _i, _p],
     'di_topk_f32': [_p, _p, _i, _i, _i, _p, _i, _p],

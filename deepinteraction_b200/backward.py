@@ -1037,3 +1037,259 @@ class DecoderPPLossFunction(torch.autograd.Function):
         g = grad.reshape(1).float().expand(2 + 2 * L).contiguous()
         r = decoder_pp_backward(ctx.dec, pts_conv, new_pts, img, *ctx.args, grad_losses=g)
         return None, r['d_pts_conv'], r['d_new_pts'], r['d_img'], None, None, None
+
+
+# ---- the ++ encoder: FusionTransformerv4 -----------------------------------------------------------------------------
+def _tr(cache, key, w):
+    """_transposed(w), built once per pack under `key` of the pack's cache dict."""
+    if key not in cache:
+        cache[key] = _transposed(w)
+    return cache[key]
+
+
+def _msda_backward(ap, sv, dy, B, hq, wq, R, prefix):
+    """Backward of msda_forward (out = output_proj(msdeform(value_proj(maps), raw(q))) + q) from its saved values ->
+    (d q rows, [d map rows per level]).  The fused raw weight's gradient is split back into sampling_offsets.* and
+    attention_weights.*; value_proj's gradient sums over the levels."""
+    cache = ap.setdefault('_bw', {})
+    _put(R, (prefix + 'output_proj', _layer_grads(dy, sv['a'])))
+    da = ops.linear([dy], _tr(cache, 'out', ap['out'][0]))
+    d_raw, d_vals = ops.msdeform_bwd(sv['vals'], sv['raw'], da, B, hq, wq, ap['heads'], ap['points'])
+    dW, db = _layer_grads(d_raw, sv['q'])
+    n_off = ap['heads'] * ap['L'] * ap['points'] * 2
+    R[prefix + 'sampling_offsets.weight'], R[prefix + 'sampling_offsets.bias'] = dW[:n_off], db[:n_off]
+    R[prefix + 'attention_weights.weight'], R[prefix + 'attention_weights.bias'] = dW[n_off:], db[n_off:]
+    d_q = ops.linear([d_raw], _tr(cache, 'raw', ap['raw'][0]), res=dy)
+    dWv = dbv = None
+    d_maps = []
+    for m, dv in zip(sv['maps'], d_vals):
+        C = m.shape[-1]
+        dWl, dbl = _layer_grads(dv.view(-1, C), m.reshape(-1, C))
+        dWv, dbv = _add(dWv, dWl), _add(dbv, dbl)
+        d_maps.append(ops.linear([dv.view(-1, C)], _tr(cache, 'value', ap['value'][0])))
+    _put(R, (prefix + 'value_proj', (dWv, dbv)))
+    return d_q, d_maps
+
+
+def _ffn_backward(pk, sv, dy, cache, key, R, prefix):
+    """Backward of ffn_forward (out = linear2(relu(linear1(x))) + x) -> d x; parameter gradients into R."""
+    w1, _, w2, _ = pk
+    _put(R, (prefix + 'layers.1', _layer_grads(dy, sv['h'])))
+    dh = ops.relu_bwd(ops.linear([dy], _tr(cache, key + '2', w2)), sv['h'])
+    _put(R, (prefix + 'layers.0.0', _layer_grads(dh, sv['x'])))
+    return ops.linear([dh], _tr(cache, key + '1', w1), res=dy)
+
+
+def _polar_backward(ap, sv, dy, R, prefix):
+    """Backward of polar.polar_forward from d out [B*Y*X, C] rows -> (d lidar rows (the residual, plus the ray queries'
+    sampling), d image-map rows (through the memory)).  The block is evaluated in fp32 as its forward, dropout off."""
+    cache = ap.setdefault('_bw', {})
+    C = dy.shape[1]
+    BV, Rr, w, _ = sv['rays_shape']
+    h = sv['cols'].shape[0] // (BV * w)
+    T = 'transformer_layers.'
+    D = prefix + T + 'decoder.layers.0.'
+    sa, ca = ap['self_attn'], ap['cross']
+    d_lidar = dy.contiguous()
+    proj, undo, camc, V, in_hw, pc, r0, r_cnt = sv['gather']
+    bev = sv['bev_shape']
+    d_x4 = ops.polar_gather_bwd(d_lidar.view(bev), sv['rays_shape'], proj, undo, camc, V, in_hw, pc, r0, r_cnt)
+    d_x3, R[prefix + T + 'decoder.norm.weight'], R[prefix + T + 'decoder.norm.bias'] = ops.ln_bwd(
+        d_x4.view(-1, C), sv['x3'], ap['dec_norm'][0])
+    w1, _, w2, _ = ap['ffn']
+    d_x2, n3, l2, l1 = _ffn_norm_backward(d_x3, sv['z3'], ap['norm3'][0], sv['f'], (ops.relu_bwd, sv['f']), sv['x2'],
+                                          _tr(cache, 'ffn2', w2), _tr(cache, 'ffn1', w1))
+    _put(R, (D + 'norm3', n3), (D + 'linear2', l2), (D + 'linear1', l1))
+    # norm2, cross attention over the image column (memory)
+    dz2, R[D + 'norm2.weight'], R[D + 'norm2.bias'] = ops.ln_bwd(d_x2, sv['z2'], ap['norm2'][0])
+    _put(R, (D + 'multihead_attn.out_proj', _layer_grads(dz2, sv['a2'])))
+    da2 = ops.linear([dz2], _tr(cache, 'cross_out', ca['out'][0]))
+    kv = sv['kv']
+    dq2 = torch.empty_like(sv['q2'])
+    dkv = torch.empty_like(kv)
+    ops.seq_attn_bwd(sv['q2'], kv[:, :C], kv[:, C:], sv['a2'], da2, BV, w, Rr, h, ap['heads'], dq2, dkv[:, :C], dkv[:, C:])
+    dWq, dbq = _layer_grads(dq2, sv['x1'])
+    dWkv, dbkv = _layer_grads(dkv, sv['memory'])
+    R[D + 'multihead_attn.in_proj_weight'] = torch.cat([dWq, dWkv], 0)
+    R[D + 'multihead_attn.in_proj_bias'] = torch.cat([dbq, dbkv], 0)
+    d_x1 = ops.linear([dq2], _tr(cache, 'cross_q', ca['q'][0]), res=dz2)
+    d_mem = ops.linear([dkv], _tr(cache, 'cross_kv', ca['kv'][0]))
+    d_cols, R[prefix + T + 'encoder.norm.weight'], R[prefix + T + 'encoder.norm.bias'] = ops.ln_bwd(
+        d_mem, sv['cols'], ap['enc_norm'][0])
+    # norm1, self attention along the ray
+    dz1, R[D + 'norm1.weight'], R[D + 'norm1.bias'] = ops.ln_bwd(d_x1, sv['z1'], ap['norm1'][0])
+    _put(R, (D + 'self_attn.out_proj', _layer_grads(dz1, sv['a1'])))
+    da1 = ops.linear([dz1], _tr(cache, 'self_out', sa['out'][0]))
+    qkv = sv['qkv']
+    dqkv = torch.empty_like(qkv)
+    ops.seq_attn_bwd(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], sv['a1'], da1, BV, w, Rr, Rr, ap['heads'],
+                     dqkv[:, :C], dqkv[:, C:2 * C], dqkv[:, 2 * C:])
+    R[D + 'self_attn.in_proj_weight'], R[D + 'self_attn.in_proj_bias'] = _layer_grads(dqkv, sv['rays'])
+    d_rays = ops.linear([dqkv], _tr(cache, 'self_in', sa['qkv'][0]), res=dz1)
+    d_bev = ops.bev_sample_bwd(d_rays.view(BV, Rr, w, C), sv['grid'], V, bev)
+    return _add(d_lidar, d_bev.view(-1, C)), d_cols
+
+
+def _pp_cross_backward(layer, ap, idx, sv, dy, ctx, R, prefix):
+    """Backward of FusionTransformerv4._cross -> (d query rows, d value-map rows or None)."""
+    C = dy.shape[1]
+    g = ctx['g']
+    if ap['kind'] == 'p2i':             # 1-level MSDA over the BEV map sampled at the warp grid
+        Bq, hq, wq, _ = sv['maps'][0].shape
+        d_q, (d_warped,) = _msda_backward(ap, sv, dy, Bq, hq, wq, R, prefix + 'Local.')
+        d_bev = ops.bev_sample_bwd(d_warped.view(Bq, hq, wq, C), g.grid, g.V, sv['value_shape'])
+        return d_q, d_bev.view(-1, C)
+    if ap['kind'] == 'i2p':             # + residual (:364)
+        qm = sv['query_map']
+        r = i2p_backward(ap['w'], qm, sv['value_map'], ctx['pm'], g.proj, g.V, g.in_hw, dy.view(qm.shape))
+        mha = layer.attentions[idx].learnedAlign
+        with fold.on_device():
+            u = fold.i2p_unfold_grads(mha, r['dM1'], r['dc1'], r['dM2'], r['dc2'])
+        f32 = lambda *ts: torch.cat(ts, 0).float()
+        A = prefix + 'learnedAlign.'
+        R[A + 'in_proj_weight'], R[A + 'in_proj_bias'] = f32(u['Wq'], u['Wk'], u['Wv']), f32(u['bq'], u['bk'], u['bv'])
+        R[A + 'out_proj.weight'], R[A + 'out_proj.bias'] = u['Wo'].float(), u['bo'].float()
+        return _add(dy, r['d_pts'].view(-1, C)), r['d_img'].view(-1, C)
+    return _polar_backward(ap, sv, dy, R, prefix)
+
+
+def _pp_layer_backward(layer, lp, sv, d_out, ctx, R, prefix):
+    """Backward of FusionTransformerv4._layer from its saved tape: d out rows -> (d query rows, d value-map rows or
+    None, [d multi-scale map rows per level or None]).  out = self_feat + scale * query; self_feat is the self
+    attention's output, so the gradient of its branch joins the query's there."""
+    cache = lp.setdefault('_bw', {})
+    d_q, R[prefix + 'scale'] = ops.axpy_bwd(d_out, sv['query'], lp['scale'])
+    grads = dict(query=d_q, self=d_out)
+    Bq, hq, wq, _ = sv['shape']
+    d_value, d_ms = None, None
+    for op, idx, stream, s in reversed(sv['tape']):
+        gr = grads[stream]
+        if op == 'self_attn':
+            gr = _add(gr, grads['self'])
+            grads['self'] = None
+            gr, d_maps = _msda_backward(lp['attn'][idx], s, gr, Bq, hq, wq, R, prefix + 'attentions.%d.' % idx)
+            d_ms = d_maps if d_ms is None else [_add(a, b) for a, b in zip(d_ms, d_maps)]
+        elif op == 'norm':
+            gr, R[prefix + 'norms.%d.weight' % idx], R[prefix + 'norms.%d.bias' % idx] = ops.ln_bwd(gr, s['x'], lp['norms'][idx][0])
+        elif op == 'ffn':
+            gr = _ffn_backward(lp['ffns'][idx], s, gr, cache, 'ffn%d.' % idx, R, prefix + 'ffns.%d.' % idx)
+        else:
+            gr, dv = _pp_cross_backward(layer, lp['attn'][idx], idx, s, gr, ctx, R, prefix + 'attentions.%d.' % idx)
+            d_value = _add(d_value, dv)
+        grads[stream] = gr
+    return grads['query'], d_value, d_ms
+
+
+def _encoder_pp_checks(enc, img_levels, pts_levels, d_img, d_pts_conv, d_pts):
+    """NotImplementedError before any launch for what encoder_pp_backward does not cover."""
+    from . import mmri_pp
+    if not isinstance(enc, mmri_pp.FusionTransformerv4):
+        raise NotImplementedError('encoder_pp_backward covers the ++ encoder mmri_pp.FusionTransformerv4 only (the base '
+                                  f'DeepInteractionEncoder: encoder_backward; got {type(enc).__name__})')
+    C = enc.hidden_channel
+    if C != 128:
+        raise NotImplementedError(f'encoder_pp_backward: the gradient kernels take hidden_channel = 128 (got {C})')
+    for blocks in (enc.img_fusion_blocks, enc.pts_fusion_blocks):
+        for layer in blocks:
+            for a in layer.attentions:
+                m = a.Local if isinstance(a, mmri_pp.MMRI_P2I) else a
+                if isinstance(m, mmri_pp.MultiScaleDeformableAttention) and not (
+                        m.num_heads == 8 and m.num_points == 4 and m.num_levels in (1, 2) and m.embed_dims == 128):
+                    raise NotImplementedError('encoder_pp_backward: the deformable-attention gradient takes 8 heads, 4 points '
+                                              f'and 1 or 2 levels (got {m.num_heads}, {m.num_points}, {m.num_levels})')
+    img_levels, pts_levels = list(img_levels), list(pts_levels)
+    lv = lambda blocks: {a.num_levels for l in blocks for a in l.attentions if isinstance(a, mmri_pp.MultiScaleDeformableAttention)}
+    if lv(enc.img_fusion_blocks) != {len(img_levels)} or lv(enc.pts_fusion_blocks) != {len(pts_levels) - 1}:
+        raise NotImplementedError(f'encoder_pp_backward: {len(img_levels)} image and {len(pts_levels)} point-cloud levels do '
+                                  'not match the layers (self attention over every image level and every point-cloud level '
+                                  'after the first)')
+    ci, cp, cs = (enc.multi_scale_conv_img.in_channels, enc.multi_scale_conv_pts.in_channels,
+                  enc.shared_conv_pts.in_channels)
+    shapes = [tuple(t.shape) for t in img_levels + pts_levels]
+    B = pts_levels[0].shape[0] if pts_levels[0].dim() == 4 else 0
+    ok = (all(t.dim() == 4 for t in img_levels + pts_levels) and B > 0 and img_levels[0].shape[0] % B == 0
+          and all(t.shape[1] == ci and t.shape[0] == img_levels[0].shape[0] for t in img_levels)
+          and pts_levels[0].shape[1] == cs
+          and all(t.shape[1] == cp and t.shape[0] == B and t.shape[2:] == pts_levels[0].shape[2:] for t in pts_levels[1:]))
+    if ok:
+        BV, _, h, w = img_levels[0].shape
+        _, _, Y, X = pts_levels[0].shape
+        want = ((d_img, (BV, h, w, C)), (d_pts_conv, (B, Y, X, C)), (d_pts, (B, Y, X, C)))
+        ok = all(d is None or tuple(d.shape) == s for d, s in want)
+    if not ok:
+        raise NotImplementedError(f'encoder_pp_backward: image levels [B*V, {ci}, h, w], point-cloud levels [B, {cs}, Y, X] '
+                                  f'then [B, {cp}, Y, X], output gradients [B*V, h, w, {C}] / [B, Y, X, {C}] pixel-major '
+                                  f'(got {shapes})')
+
+
+@_precise()
+def encoder_pp_backward(enc, img_levels, pts_levels, img_metas, pts_metas, d_img, d_pts_conv, d_pts):
+    """Backward of the ++ encoder FusionTransformerv4.forward (reference fusion_transformerv4.py:25-640) with dropout off;
+    it has no BatchNorm, so this is the training gradient of the neck.  img_levels [B*V, Ci, h_l, w_l] and pts_levels
+    ([B, 2 Cp, Y, X] concat, then [B, Cp, Y, X] maps): the module's NCHW inputs on the GPU; pts_metas with pillars;
+    d_img [B*V, h, w, C], d_pts_conv / d_pts [B, Y, X, C]: gradients of the three outputs, pixel-major (None = zero;
+    decoder_pp_backward's d_img, d_pts_conv, d_new_pts).
+    -> dict(d_img_levels, d_pts_levels: pixel-major [N, H, W, C_in] per input level, grads = {name: tensor} keyed and
+    shaped as enc.state_dict(), every parameter present).  The forward is re-run eagerly (FusionTransformerv4._schedule
+    with saved=) and its operation tape walked in reverse; both layers' self attentions read the same multi-scale maps, so
+    their value gradients add up per level.  Everything stays on the device, without host synchronisation after the
+    first call of a pack (pts_metas given on the device)."""
+    _encoder_pp_checks(enc, img_levels, pts_levels, d_img, d_pts_conv, d_pts)
+    pk = enc.pack()
+    C = enc.hidden_channel
+    img_levels, pts_levels = [t.contiguous() for t in img_levels], [t.contiguous() for t in pts_levels]
+    dev = img_levels[0].device
+    pillars, coors, npts, pts_list, consts = enc._frame(img_metas, pts_metas, dev)
+    pm = dict(pillars=pillars, pillar_coors=coors, pillars_num_points=npts, pts=pts_list)
+    # pinned sources keep the uploads asynchronous; no live counts: the point arrays have their exact sizes
+    consts = [c.pin_memory().to(dev, non_blocking=True) for c in consts] + [None]
+    sv = {}
+    img, pts_conv, pts = enc._schedule(img_levels, pts_levels, img_metas, pm, consts, saved=sv)
+    ctx = sv['ctx']
+    R = {}
+    gi, gp = _seed_rows(d_img, img), _seed_rows(d_pts, pts)
+    d_ms_img = d_ms_pts = None
+    add_all = lambda acc, new: new if acc is None else [_add(a, b) for a, b in zip(acc, new)]
+    for i in reversed(range(enc.num_layers)):
+        # t_pts reads (new_pts, new_img) and t_img reads (new_img, new_pts) of the previous layer
+        dq_p, dv_p, dms_p = _pp_layer_backward(enc.pts_fusion_blocks[i], pk['pts'][i], sv['pts'][i], gp, ctx, R,
+                                               'pts_fusion_blocks.%d.' % i)
+        dq_i, dv_i, dms_i = _pp_layer_backward(enc.img_fusion_blocks[i], pk['img'][i], sv['img'][i], gi, ctx, R,
+                                               'img_fusion_blocks.%d.' % i)
+        d_ms_img, d_ms_pts = add_all(d_ms_img, dms_i), add_all(d_ms_pts, dms_p)
+        gi, gp = _add(dq_i, dv_p), _add(dq_p, dv_i)
+    d_ms_img[0], d_ms_pts[0] = _add(d_ms_img[0], gi), _add(d_ms_pts[0], gp)     # level 0 is the first layer's query
+
+    def convs(name, xs, gs):
+        dxs, dW, db = [], None, None
+        for x, g in zip(xs, gs):
+            dx, (w, b) = _shared_conv_backward(g.contiguous(), pk[name][0], x)
+            dxs.append(dx)
+            dW, db = _add(dW, w), _add(db, b)
+        R[name + '.weight'], R[name + '.bias'] = dW, db
+        return dxs
+    d_img_levels = convs('multi_scale_conv_img', img_levels, d_ms_img)
+    d_pts_levels = (convs('shared_conv_pts', pts_levels[:1], [_seed_rows(d_pts_conv, pts_conv)])
+                    + convs('multi_scale_conv_pts', pts_levels[1:], d_ms_pts))
+    return dict(d_img_levels=d_img_levels, d_pts_levels=d_pts_levels, grads=R)
+
+
+class EncoderPPFunction(torch.autograd.Function):
+    """autograd wrapper: EncoderPPFunction.apply(enc, img_metas, pts_metas, n_img, *img_levels, *pts_levels) ->
+    (img [B*V, h, w, C], pts_conv, pts [B, Y, X, C]) = enc.forward_nhwc(...) with the forward schedule's kernels;
+    backward -> the input levels' gradients in their NCHW layout through encoder_pp_backward.  Parameter gradients are
+    returned by encoder_pp_backward."""
+
+    @staticmethod
+    def forward(ctx, enc, img_metas, pts_metas, n_img, *levels):
+        _encoder_pp_checks(enc, levels[:n_img], levels[n_img:], None, None, None)
+        ctx.enc, ctx.metas, ctx.n_img = enc, (img_metas, pts_metas), n_img
+        ctx.save_for_backward(*levels)
+        return enc.forward_nhwc(list(levels[:n_img]), list(levels[n_img:]), img_metas, pts_metas)
+
+    @staticmethod
+    def backward(ctx, d_img, d_pts_conv, d_pts):
+        levels, n = ctx.saved_tensors, ctx.n_img
+        r = encoder_pp_backward(ctx.enc, levels[:n], levels[n:], *ctx.metas, d_img, d_pts_conv, d_pts)
+        grads = [ops.nhwc_to_nchw(d.contiguous()) for d in r['d_img_levels'] + r['d_pts_levels']]
+        return (None, None, None, None) + tuple(grads)

@@ -167,18 +167,25 @@ def _pack_ln(m, device):
     return fold.dev(m.weight.detach().double().cpu(), device), fold.dev(m.bias.detach().double().cpu(), device), float(m.eps)
 
 
-def msda_forward(pk, query_rows, value_maps, B, hq, wq):
-    """mmcv MultiScaleDeformableAttention.forward (identity = query, batch_first): value_maps = list of [B,H_l,W_l,C]."""
+def msda_forward(pk, query_rows, value_maps, B, hq, wq, saved=None):
+    """mmcv MultiScaleDeformableAttention.forward (identity = query, batch_first): value_maps = list of [B,H_l,W_l,C].
+    saved (a dict) receives the query rows, the value maps, their projections, raw and the sampled rows."""
     C = query_rows.shape[1]
     vals = [ops.linear([v.view(-1, C)], *pk['value']).view(v.shape) for v in value_maps]
     raw = ops.linear([query_rows], *pk['raw'])
     a = ops.msdeform(vals, raw, B, hq, wq, pk['heads'], pk['points'])
+    if saved is not None:
+        saved.update(q=query_rows, maps=list(value_maps), vals=vals, raw=raw, a=a)
     return ops.linear([a], *pk['out'], res=query_rows)
 
 
-def ffn_forward(pk, x):
+def ffn_forward(pk, x, saved=None):
+    """FFN (identity = x); saved (a dict) receives the input and the hidden rows."""
     w1, b1, w2, b2 = pk
-    return ops.linear([ops.linear([x], w1, b1, ops.ACT_RELU)], w2, b2, res=x)
+    h = ops.linear([x], w1, b1, ops.ACT_RELU)
+    if saved is not None:
+        saved.update(x=x, h=h)
+    return ops.linear([h], w2, b2, res=x)
 
 
 def ln_forward(pk, x):
@@ -247,46 +254,69 @@ class FusionTransformerv4(nn.Module):
         return pk
 
     # -- forward -----------------------------------------------------------------------------------
-    def _layer(self, lp, query_map, value_map, ms_maps, ctx):
-        """DeepInteractionLayer.forward (:161-218) on pixel-major maps.  query_map [Bq,hq,wq,C] (Bq = B*V or B)."""
+    def _layer(self, lp, query_map, value_map, ms_maps, ctx, saved=None):
+        """DeepInteractionLayer.forward (:161-218) on pixel-major maps.  query_map [Bq,hq,wq,C] (Bq = B*V or B).
+        saved (a dict) selects the eager re-run of backward.encoder_pp_backward: saved['tape'] then lists every applied
+        operation as (op, module index, 'query' or 'self' (the self_feat branch), its saved values), in order; the
+        returned map is the same either way."""
         Bq, hq, wq, C = query_map.shape
         query = query_map.view(-1, C)
         order = lp['order']
         ni = ai = fi = 0
         self_feat = None
+        tape = None if saved is None else saved.setdefault('tape', [])
         for op in order[:-2]:
+            sv = None if saved is None else {}
+            idx = None
             if op == 'self_attn':
-                query = msda_forward(lp['attn'][ai], query, ms_maps, Bq, hq, wq)
+                query, idx = msda_forward(lp['attn'][ai], query, ms_maps, Bq, hq, wq, saved=sv), ai
                 ai += 1
                 self_feat = query
             elif op == 'norm':
-                query = ln_forward(lp['norms'][ni], query)
+                if sv is not None:
+                    sv['x'] = query
+                query, idx = ln_forward(lp['norms'][ni], query), ni
                 ni += 1
             elif op == 'cross_attn':
-                query = self._cross(lp['attn'][ai], query.view(Bq, hq, wq, C), value_map, ctx).view(-1, C)
+                query = self._cross(lp['attn'][ai], query.view(Bq, hq, wq, C), value_map, ctx, saved=sv).view(-1, C)
+                idx = ai
                 ai += 1
             elif op == 'ffn':
-                query = ffn_forward(lp['ffns'][fi], query)
+                query, idx = ffn_forward(lp['ffns'][fi], query, saved=sv), fi
                 fi += 1
+            if tape is not None and idx is not None:
+                tape.append((op, idx, 'query', sv))
         for op in order[-2:]:
+            sv = None if saved is None else {}
+            idx = None
             if op == 'norm':
-                self_feat = ln_forward(lp['norms'][ni], self_feat)
+                if sv is not None:
+                    sv['x'] = self_feat
+                self_feat, idx = ln_forward(lp['norms'][ni], self_feat), ni
                 ni += 1
             elif op == 'ffn':
-                self_feat = ffn_forward(lp['ffns'][fi], self_feat)
+                self_feat, idx = ffn_forward(lp['ffns'][fi], self_feat, saved=sv), fi
                 fi += 1
+            if tape is not None and idx is not None:
+                tape.append((op, idx, 'self', sv))
+        if saved is not None:
+            saved.update(self_feat=self_feat, query=query, shape=(Bq, hq, wq, C))
         return ops.axpy(self_feat, query, lp['scale']).view(Bq, hq, wq, C)
 
-    def _cross(self, ap, query_map, value_map, ctx):
+    def _cross(self, ap, query_map, value_map, ctx, saved=None):
         g, pm, counts = ctx['g'], ctx['pm'], ctx['counts']
         Bq, hq, wq, C = query_map.shape
         if ap['kind'] == 'p2i':            # query = image maps [B*V,h,w,C], value = BEV map [B,Y,X,C]
             g.wait()
             warped = ops.bev_sample(value_map, g.grid, g.V)
-            return msda_forward(ap, query_map.view(-1, C), [warped], Bq, hq, wq).view(Bq, hq, wq, C)
+            if saved is not None:
+                saved['value_shape'] = tuple(value_map.shape)
+            return msda_forward(ap, query_map.view(-1, C), [warped], Bq, hq, wq, saved=saved).view(Bq, hq, wq, C)
         if ap['kind'] == 'i2p':            # query = BEV map, value = image maps; + residual (:364)
             n_dev = None if counts is None else counts[0:1]
             coors = pm['pillar_coors']
+            if saved is not None:
+                saved.update(query_map=query_map, value_map=value_map)
             out = query_map.clone()
             if coors.shape[0] == 0:
                 return out
@@ -298,7 +328,7 @@ class FusionTransformerv4(nn.Module):
             return ops.scatter_rows_add(o, cnt, coors, out, n_dev)
         if ap['kind'] == 'polar':
             from .polar import polar_forward
-            return polar_forward(ap, query_map, value_map, ctx)
+            return polar_forward(ap, query_map, value_map, ctx, saved=saved)
         raise NotImplementedError(ap['kind'])
 
     def forward_nhwc(self, img_feats, pts_feats, img_metas, pts_metas):
@@ -310,16 +340,7 @@ class FusionTransformerv4(nn.Module):
         self.pack()
         img_feats, pts_feats = [t.contiguous() for t in img_feats], [t.contiguous() for t in pts_feats]
         dev_ = img_feats[0].device
-        pillars = pts_metas['pillars'].to(device=dev_, dtype=torch.float32).contiguous()
-        coors = pts_metas['pillar_coors'].to(device=dev_, dtype=torch.int32).contiguous()
-        npts = pts_metas['pillars_num_points'].to(device=dev_, dtype=torch.int32).contiguous()
-        pts_list = [p.to(device=dev_, dtype=torch.float32) for p in pts_metas['pts']]
-        proj_h, i2l_h = geom.camera_rows_host(img_metas)
-        consts = [proj_h, i2l_h]
-        has_polar = any(a['kind'] == 'polar' for l in self._pack['pts'] for a in l['attn'])
-        if has_polar:
-            from .polar import polar_consts_host
-            consts += list(polar_consts_host(img_metas))
+        pillars, coors, npts, pts_list, consts = self._frame(img_metas, pts_metas, dev_)
         B_, _, Y_, X_ = pts_feats[0].shape
         staged = [pillars, coors, npts] + pts_list
         caps = [_pow2_cap(pillars.shape[0], B_ * Y_ * X_)] * 3 + [_pow2_cap(p.shape[0], POINT_CAP_MIN) for p in pts_list]
@@ -334,7 +355,24 @@ class FusionTransformerv4(nn.Module):
             return self._schedule(list(ins[:n_img]), list(ins[n_img:]), img_metas, pm, cs)
         return self._graphs.run(sig, inputs, consts, fn, staged=staged, caps=caps)
 
-    def _schedule(self, img_feats, pts_feats, img_metas, pm, consts):
+    def _frame(self, img_metas, pts_metas, dev_):
+        """-> (pillars, coors, npts, pts list) on the device in the schedule's dtypes, and the frame's host constants:
+        the camera rows and, when a layer has a polar block, its constants (polar.polar_consts_host)."""
+        pillars = pts_metas['pillars'].to(device=dev_, dtype=torch.float32).contiguous()
+        coors = pts_metas['pillar_coors'].to(device=dev_, dtype=torch.int32).contiguous()
+        npts = pts_metas['pillars_num_points'].to(device=dev_, dtype=torch.int32).contiguous()
+        pts_list = [p.to(device=dev_, dtype=torch.float32) for p in pts_metas['pts']]
+        proj_h, i2l_h = geom.camera_rows_host(img_metas)
+        consts = [proj_h, i2l_h]
+        if any(a['kind'] == 'polar' for l in self._pack['pts'] for a in l['attn']):
+            from .polar import polar_consts_host
+            consts += list(polar_consts_host(img_metas))
+        return pillars, coors, npts, pts_list, consts
+
+    def _schedule(self, img_feats, pts_feats, img_metas, pm, consts, saved=None):
+        """The kernel schedule.  consts: device tensors (camera rows, polar constants when present, then the live counts
+        or None for exact-size point arrays).  saved (a dict) selects the eager re-run of backward.encoder_pp_backward:
+        it receives the geometry, the context, the multi-scale maps and per layer the saved dict of _layer."""
         pk = self._pack
         dev_ = img_feats[0].device
         C = self.hidden_channel
@@ -355,9 +393,15 @@ class FusionTransformerv4(nn.Module):
         ctx = dict(g=g, pm=pm, counts=counts, img_metas=img_metas, B=B, V=BV // B)
         if len(consts) > 3:
             ctx['polar_consts'] = tuple(consts[2:5])
+        if saved is not None:
+            saved.update(g=g, ctx=ctx, ms_img=ms_img, ms_pts=ms_pts, pts_conv=pts_conv, img=[], pts=[])
         for i in range(self.num_layers):
-            t_img = self._layer(pk['img'][i], new_img, new_pts, ms_img, ctx)
-            t_pts = self._layer(pk['pts'][i], new_pts, new_img, ms_pts, ctx)
+            s_img, s_pts = (None, None) if saved is None else ({}, {})
+            if saved is not None:
+                saved['img'].append(s_img)
+                saved['pts'].append(s_pts)
+            t_img = self._layer(pk['img'][i], new_img, new_pts, ms_img, ctx, saved=s_img)
+            t_pts = self._layer(pk['pts'][i], new_pts, new_img, ms_pts, ctx, saved=s_pts)
             new_img, new_pts = t_img, t_pts
         return new_img, pts_conv, new_pts
 

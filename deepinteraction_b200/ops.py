@@ -380,6 +380,57 @@ def axpy(a, b, scale):
     return out
 
 
+def msdeform_bwd(values, raw, dout, B, hq, wq, heads=8, points=4):
+    """Gradient of msdeform: dout [B*hq*wq, C] -> (d_raw [B*hq*wq, heads*L*P*3] in raw's layout (offsets | logits),
+    [d value_l [B, H_l, W_l, C]])."""
+    L = len(values)
+    C = values[0].shape[-1]
+    assert all(v.is_contiguous() and v.shape[0] == B for v in values) and raw.shape[0] == B * hq * wq
+    d_raw = torch.empty(raw.shape[0], heads * L * points * 3, device=raw.device, dtype=torch.float32)
+    d_vals = [torch.zeros_like(v) for v in values]
+    sh = (ctypes.c_int * (2 * L))(*[d for v in values for d in v.shape[1:3]])
+    (pr, ldr), (pd, ldd) = _rows(raw), _rows(dout)
+    _call('di_msdeform_bwd_f32', _ptr(values[0]), _ptr(values[1]) if L > 1 else None, pr, ldr, pd, ldd, _ptr(d_raw),
+          d_raw.stride(0), _ptr(d_vals[0]), _ptr(d_vals[1]) if L > 1 else None, B, hq * wq, hq, wq, heads, C // heads, L,
+          points, sh, _stream(), nbytes=4 * (2 * sum(v.numel() for v in values) + raw.numel() + d_raw.numel() + dout.numel()))
+    return d_raw, d_vals
+
+
+def seq_attn_bwd(q, k, v, out, dout, G, Wn, Lq, Lk, heads, dq, dk, dv):
+    """Gradient of seq_attn from its saved output `out`: dout [G*Lq*Wn, C] -> dq, dk, dv written into the given row views
+    (e.g. the three column blocks of one packed [M, 3C] buffer)."""
+    C = q.shape[1]
+    args = []
+    for t in (q, k, v, out, dout, dq, dk, dv):
+        args += list(_rows(t))
+    _call('di_seq_attn_bwd_f32', *args, G, Wn, Lq, Lk, heads, C // heads, _stream(), flops=10 * G * Wn * Lq * Lk * C)
+    return dq, dk, dv
+
+
+def polar_gather_bwd(d_out, rays_shape, proj, undo, camc, V, in_hw, pc_range, r0, r_count):
+    """Adjoint of polar_gather w.r.t. the rays: d_out [B, Y, X, C] -> d_rays of shape rays_shape [B*V, R, W, C]."""
+    BV, R, W, C = rays_shape
+    B, Y, X, _ = d_out.shape
+    assert d_out.is_contiguous()
+    d_rays = torch.zeros(BV, R, W, C, device=d_out.device, dtype=torch.float32)
+    rng = (ctypes.c_float * 6)(*[float(v) for v in pc_range])
+    _call('di_polar_gather_bwd_f32', _ptr(d_out), _ptr(proj), _ptr(undo), _ptr(camc), _ptr(d_rays), B, V, R, W, Y, X, C,
+          in_hw[0], in_hw[1], rng, float(r0), float(r_count), _stream(), nbytes=4 * (2 * d_rays.numel() + d_out.numel()))
+    return d_rays
+
+
+def axpy_bwd(dout, b, scale):
+    """Gradient of axpy(a, b, scale) w.r.t. b and scale: -> (s * dout, d scale [1] = sum dout . b); d a is dout."""
+    assert dout.is_contiguous() and b.is_contiguous() and dout.shape == b.shape
+    n = _lib.check(_lib.lib().di_axpy_bwd_workspace(), 'di_axpy_bwd_workspace')
+    work = torch.empty(n, device=b.device, dtype=torch.float64)
+    db = torch.empty_like(b)
+    ds = torch.empty(1, device=b.device, dtype=torch.float32)
+    _call('di_axpy_bwd_f32', _ptr(dout), _ptr(b), _ptr(scale), _ptr(db), _ptr(ds), _ptr(work), b.numel(), _stream(),
+          nbytes=12 * b.numel(), launches=2)
+    return db, ds
+
+
 def i2p_attend(qk, pillars, npts, coors, proj, img_nhwc, V, in_hw, n_dev=None, dropout=None):
     """dropout = (p, seed): training-mode attention dropout (mask = hash(seed, pillar, key), see i2p_dropout_mask); s is then
     [P, C + 4] with rho = sum_j a_j m_j in column C (fold.i2p_fold(split_bias=True) gives the matching [C, C + 4] weight)."""

@@ -76,8 +76,10 @@ def polar_consts_host(img_metas):
     return cam_t, torch.from_numpy(undo), cam_t[:, 8:10].contiguous()
 
 
-def polar_forward(ap, lidar_map, img_map, ctx):
-    """lidar_map [B,Y,X,C] (queries / residual), img_map [B*V,h,w,C] (memory) -> [B,Y,X,C]."""
+def polar_forward(ap, lidar_map, img_map, ctx, saved=None):
+    """lidar_map [B,Y,X,C] (queries / residual), img_map [B*V,h,w,C] (memory) -> [B,Y,X,C].  saved (a dict) receives
+    what backward.encoder_pp_backward needs: the ray grid and constants, the rows between the steps and the pre-norm
+    sums (recomputed by one more GEMM each; the returned map is the same either way)."""
     B, Y, X, C = lidar_map.shape
     BV, h, w, _ = img_map.shape
     V, R, H = BV // B, ap['R'], ap['heads']
@@ -99,14 +101,20 @@ def polar_forward(ap, lidar_map, img_map, ctx):
     memory = ln(ap['enc_norm'], cols)
     sa = ap['self_attn']
     qkv = ops.linear([rays], *sa['qkv'])
-    a = ops.seq_attn(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], BV, w, R, R, H)
-    x = ln(ap['norm1'], ops.linear([a], *sa['out']), res=rays)
+    a1 = ops.seq_attn(qkv[:, :C], qkv[:, C:2 * C], qkv[:, 2 * C:], BV, w, R, R, H)
+    x1 = ln(ap['norm1'], ops.linear([a1], *sa['out']), res=rays)
     ca = ap['cross']
-    q2 = ops.linear([x], *ca['q'])
+    q2 = ops.linear([x1], *ca['q'])
     kv = ops.linear([memory], *ca['kv'])
-    a = ops.seq_attn(q2, kv[:, :C], kv[:, C:], BV, w, R, h, H)
-    x = ln(ap['norm2'], ops.linear([a], *ca['out']), res=x)
+    a2 = ops.seq_attn(q2, kv[:, :C], kv[:, C:], BV, w, R, h, H)
+    x2 = ln(ap['norm2'], ops.linear([a2], *ca['out']), res=x1)
     w1, b1, w2, b2 = ap['ffn']
-    x = ln(ap['norm3'], ops.linear([ops.linear([x], w1, b1, ops.ACT_RELU)], w2, b2), res=x)
-    x = ln(ap['dec_norm'], x)
+    f = ops.linear([x2], w1, b1, ops.ACT_RELU)
+    x3 = ln(ap['norm3'], ops.linear([f], w2, b2), res=x2)
+    if saved is not None:
+        saved.update(grid=grid, bev_shape=(B, Y, X, C), rays_shape=(BV, R, w, C), cols=cols, rays=rays, qkv=qkv, a1=a1,
+                     z1=ops.linear([a1], *sa['out'], res=rays), x1=x1, q2=q2, memory=memory, kv=kv, a2=a2,
+                     z2=ops.linear([a2], *ca['out'], res=x1), x2=x2, f=f, z3=ops.linear([f], w2, b2, res=x2), x3=x3,
+                     gather=(g.proj, undo, camc, V, g.in_hw, ap['pc_range'], rr[0], float(R)))
+    x = ln(ap['dec_norm'], x3)
     return ops.polar_gather(x.view(BV, R, w, C), lidar_map, g.proj, undo, camc, V, g.in_hw, ap['pc_range'], rr[0], float(R))

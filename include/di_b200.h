@@ -236,6 +236,29 @@ int di_polar_gather_f32(const float* rays, const float* lidar, const float* proj
                         float* out, int B, int V, int R, int W, int Y, int X, int C, int H_in, int W_in,
                         const float* pc_range, float r0, float r_count, cudaStream_t stream);
 
+/* Backward of the ++ encoder's kernels (deform.cu).
+ * di_msdeform_bwd_f32: gradient of di_msdeform_f32 (same inputs and configuration; -3 for the same unsupported ones):
+ *   dout [B*NQ, ldo] -> d_raw [B*NQ, ld_draw] in raw's layout (written without atomics: the same bits on every call),
+ *   d_value0 / d_value1 [B, H_l, W_l, 128] += value-map gradients (zero them first).
+ * di_seq_attn_bwd_f32: gradient of di_seq_attn_f32 from its saved output out: dq, dk, dv written into row views
+ *   (strides as the forward's); Lq <= 128 (-3 otherwise), any Lk; no atomics.
+ * di_polar_gather_bwd_f32: d_rays [B*V, R, W, 128] += adjoint of di_polar_gather_f32 applied to d_out [B, Y, X, 128]
+ *   (zero d_rays first; the residual's gradient is d_out).
+ * di_axpy_bwd_f32: gradient of di_axpy_f32 w.r.t. b and scale: db = scale[0] dout, ds[0] = sum dout . b (device scalar);
+ *   work: di_axpy_bwd_workspace() doubles; block partials in double, summed in a fixed order. */
+int di_msdeform_bwd_f32(const float* value0, const float* value1, const float* raw, int ld_raw, const float* dout, int ldo,
+                        float* d_raw, int ld_draw, float* d_value0, float* d_value1, int B, int NQ, int Hq, int Wq,
+                        int heads, int dim, int L, int P, const int* shapes, cudaStream_t stream);
+int di_seq_attn_bwd_f32(const float* q, int ldq, const float* k, int ldk, const float* v, int ldv, const float* out, int ldo,
+                        const float* dout, int ldd, float* dq, int lddq, float* dk, int lddk, float* dv, int lddv, int G,
+                        int Wn, int Lq, int Lk, int heads, int dim, cudaStream_t stream);
+int di_polar_gather_bwd_f32(const float* d_out, const float* proj, const float* undo, const float* camc, float* d_rays, int B,
+                            int V, int R, int W, int Y, int X, int C, int H_in, int W_in, const float* pc_range, float r0,
+                            float r_count, cudaStream_t stream);
+int di_axpy_bwd_workspace(void);
+int di_axpy_bwd_f32(const float* dout, const float* b, const float* scale, float* db, float* ds, double* work, long long n,
+                    cudaStream_t stream);
+
 /* ---- decoder (decoder.cu) ------------------------------------------------------------------------ */
 
 /* models/dense_heads/deepinteraction_decoder.py:225-239 */

@@ -7,8 +7,9 @@
 From fixed seeds: lcab_backward (self and cross attention), LCABTrain forward + backward, decoder_layer_backward,
 point_rcnn_backward, image_rcnn_backward and decoder_backward (base shapes, batch 2) run on deterministic kernels, so the SHA-256 of every
 tensor they return is written and --compare asks the two runs to agree on every hash both have (a version without one of
-the functions is compared on the others).  encoder_backward and encoder_train_step pass through
-di_i2p_attend_bwd_f32 and di_bev_sample_bwd_f32, which accumulate with atomicAdd and differ in the last bits from run to
+the functions is compared on the others).  encoder_backward, encoder_train_step and encoder_pp_backward pass through
+di_i2p_attend_bwd_f32 and di_bev_sample_bwd_f32 (the last also through the value and ray scatters of
+di_msdeform_bwd_f32 and di_polar_gather_bwd_f32), which accumulate with atomicAdd and differ in the last bits from run to
 run; their tensors are written as they are, and --compare reports per pair the largest max|a - b| / max|a| over the
 tensors.  With --spread (a second run of version A) the A-B figure has to stay within twice the A-A2 figure.  The
 train-mode gradients of the out_proj BatchNorm biases are left out of that figure: they are analytically zero (the next
@@ -109,6 +110,18 @@ def encoder_cases(d):
         else:
             yield 'encoder_train_step', train.encoder_train_step(*args, lambda a, b, c: tuple(Gs))
             yield 'encoder_train_step.dropout', train.encoder_train_step(*args, lambda a, b, c: tuple(Gs), dropout_seed=7)
+    if hasattr(backward, 'encoder_pp_backward'):
+        from deepinteraction_b200 import mmri_pp
+        from tools.make_goldens_pp import pp_frame, pp_layers, randomize_pp
+        img_l, pts_l = pp_layers(True)
+        torch.manual_seed(2100)
+        enc = mmri_pp.FusionTransformerv4(2, 2, 16, 24, 128, img_transformerlayers=img_l, pts_transformerlayers=pts_l)
+        randomize_pp(enc, 2100)
+        enc = enc.to(d).eval()
+        fr = pp_frame(2100, True)
+        pm = {k: (v.to(d) if torch.is_tensor(v) else [p.to(d) for p in v]) for k, v in fr['pts_metas'].items()}
+        yield 'encoder_pp_backward', backward.encoder_pp_backward(enc, [t.to(d) for t in fr['img_levels']],
+                                                                  [t.to(d) for t in fr['pts_levels']], fr['img_metas'], pm, *Gs)
 
 
 def run(out_dir):
